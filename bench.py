@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""bench.py -- DDIM denoise-steps/sec of the ViewCrafter hot path on B200 (contract: task brief, BASELINE.json).
+"""bench.py -- DDIM denoise-steps/sec of the ViewCrafter hot path on H100 (BASELINE.json).
 
     python bench.py --gpus 1 --steps 4 --warmup 3                 # our arm, headline workload 25x4x72x128
     python bench.py --impl reference --steps 2 --warmup 1         # the reference's algorithm on the host CPU cores
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...   # frame/CFG-sharded, N in {2,4,8}
+    python bench.py --gpus 1 --steps 4 --warmup 3 --dump-outputs DIR  # + the last timed step's outputs as DIR/<name>.npy
 
 One "step" = one DDIMSampler.p_sample_ddim: 2 U-Net forwards (cond + uncond, CFG 7.5), guidance rescale 0.7,
 v-prediction update with eta=1 noise.  Data is synthetic (random-init weights of the shipped architecture with the
@@ -39,7 +40,8 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], tflops_burst=d["bf16_tflops"], tflops_sustained=d["bf16_tflops_sustained"], src="measured")
-    return dict(hbm_gbs=6650.0, tflops_burst=1590.0, tflops_sustained=1400.0, src="fallback")
+    # NVIDIA H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense FP16 989 TFLOP/s -- upper bounds, not reached rates
+    return dict(hbm_gbs=3350.0, tflops_burst=989.0, tflops_sustained=989.0, src="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -131,7 +133,7 @@ def time_kernel(fn, reps=5):
 
 
 def kernel_rooflines(wl, device, peaks):
-    """Dominant kernels timed alone with CUDA events on the launching (current) stream; operands exceed L2 (126 MB)."""
+    """Dominant kernels timed alone with CUDA events on the launching (current) stream; operands exceed L2 (50 MB)."""
     from viewcrafter_b200 import ops
     T, H, W = wl["T"], wl["H"], wl["W"]
     M, C = T * H * W, 320
@@ -152,10 +154,10 @@ def kernel_rooflines(wl, device, peaks):
     gn_parts = gn_parts and ops.gn_from_parts_calls > n_gn0
     by_gn = 2.0 * M * C * 2                                     # algorithmic: read once + write once, fp16
     r = {
-        "roofline": {"kernel": "gemm_tap2_kernel<160> (tcgen05 cta_group::2 tap-GEMM, 3x3 conv 320->320 @%dx%dx%d)" % (T, H, W), "bound": "tensor",
+        "roofline": {"kernel": "gemm_tap_kernel<160> (wgmma tap-GEMM, 3x3 conv 320->320 @%dx%dx%d)" % (T, H, W), "bound": "tensor",
                      "achieved": fl_conv / t_conv / 1e12, "peak": peaks["tflops_burst"], "unit": "TFLOP/s",
                      "frac": fl_conv / t_conv / 1e12 / peaks["tflops_burst"], "traffic": None, "ms": t_conv * 1e3,
-                     "peak_source": peaks["src"] + " cuBLAS bf16 burst", "algorithmic_flop": fl_conv,
+                     "peak_source": peaks["src"], "algorithmic_flop": fl_conv,
                      "algorithmic_bytes": 2.0 * M * C * 2 + 9 * C * C * 2},
         "roofline_attention": {"kernel": "flash_attn_d64_kernel (spatial self-attn, %d heads, N=%d)" % (heads, H * W), "bound": "tensor",
                                "achieved": fl_att / t_att / 1e12, "peak": peaks["tflops_burst"], "unit": "TFLOP/s",
@@ -166,19 +168,6 @@ def kernel_rooflines(wl, device, peaks):
                                "achieved": by_gn / t_gn / 1e9, "peak": peaks["hbm_gbs"], "unit": "GB/s",
                                "frac": by_gn / t_gn / 1e9 / peaks["hbm_gbs"], "traffic": None, "ms": t_gn * 1e3, "algorithmic_bytes": by_gn},
     }
-    # measured DRAM traffic per launch of the same kernels/shapes, from the committed ncu --set full capture (not re-measured
-    # here: a number taken under a profiler is never a bench value, and ncu cannot run inside the timed process)
-    import glob
-    cands = sorted(glob.glob(os.path.join(ROOT, "profiles", "r0*_ncu_traffic.json")))
-    tp = cands[-1] if cands else ""                                       # the newest committed capture
-    if tp and (T, H, W) == (25, 72, 128):                                  # the capture is of the headline shapes only
-        t = json.load(open(tp))
-        if not gn_parts and "groupnorm_fused_statistics_pass" in t:
-            t["roofline_groupnorm"] = t["groupnorm_fused_statistics_pass"]
-        for k in r:
-            if k in t:
-                r[k]["traffic"] = t[k]["traffic_bytes"]
-                r[k]["traffic_source"] = t["source"].split(" (")[0] + "; " + t[k]["note"]
     return r
 
 
@@ -247,7 +236,7 @@ def cpu_config1_measured(sd_cpu):
 def gpu_parity_and_eager_baseline(wl, model, dev, sampler, run_step):
     """(1) parity at the bench workload: one U-Net forward (t = 499) of the CUDA path vs the oracle in fp32 on this GPU, with
     E_ref = |oracle under fp16 autocast - oracle fp32| beside it (SURVEY.md 8d tolerance rule: accept <= 2 E_ref);
-    (2) the same-box GPU baseline: the reference ALGORITHM in PyTorch eager on this B200 -- the oracle port under
+    (2) the same-box GPU baseline: the reference ALGORITHM in PyTorch eager on this GPU -- the oracle port under
     torch.autocast(fp16) (viewcrafter.py:98) with fused SDPA attention (the reference's xformers path, attention.py:146-190) --
     timed for whole CFG DDIM steps (2 forwards + update) with CUDA events.  /root/reference itself cannot travel to the box."""
     from oracle import lvdm_oracle as O
@@ -331,7 +320,13 @@ def main():
     ap.add_argument("--no-batch-cfg", action="store_true")
     ap.add_argument("--no-cfg-split", action="store_true", help="N > 1: pure frame sharding (every rank runs the B=2 cond+uncond forward on its frames) instead of 2-way CFG split x N/2-way frames")
     ap.add_argument("--no-graph", action="store_true", help="launch every kernel from the host instead of replaying the captured forward")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned (x_prev, pred_x0) as DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs writes the outputs of the timed CUDA path; --impl reference has none")
+    if args.dump_outputs and args.steps < 1:
+        ap.error("--dump-outputs needs --steps >= 1 (it writes what the last timed step computed)")
     wl = WORKLOADS[args.workload]
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -339,7 +334,7 @@ def main():
     metric = "DDIM denoise-steps/sec @ %sx%df" % (wl["px"], wl["T"])
     config = {"workload": "%s: latent 1x4x%dx%dx%d, CFG 7.5 (2 U-Net forwards/step), guidance_rescale 0.7, eta 1.0, 50-step uniform_trailing schedule"
                           % (args.workload, wl["T"], wl["H"], wl["W"]),
-              "l2": "working set per forward (tens of GB of activations, 2.9 GB weights) exceeds the 126 MB L2; no flush needed",
+              "l2": "working set per forward (tens of GB of activations, 2.9 GB weights) exceeds the 50 MB L2; no flush needed",
               "cfg": ("N=1: cond+uncond as one B=2 forward; the context-free prefix (input_blocks.0, init_attn, input_blocks.1 up to "
                       "attn1; 6.9 of 165.5 TFLOP) is computed once for both branches and the cross-attention K/V of the step-invariant "
                       "context are projected once per context tensor -- same outputs as two full forwards (SURVEY.md App. C.1/C.2); "
@@ -451,12 +446,18 @@ def main():
     lib.vc_reset_launch_count()
     unet_m.graph_replayed_launches = 0
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    pred_x0 = None
     with ClockSampler(local_rank) as clk:
         e0.record()
         for i in range(args.steps):
-            x, _ = run_step(x, args.warmup + i)
+            x, pred_x0 = run_step(x, args.warmup + i)
         e1.record()
         barrier()
+    if args.dump_outputs and rank == 0 and args.steps > 0:
+        # the timed path's result, as a caller of p_sample_ddim receives it; inputs, weights and noise draws are seeded
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, t in (("x_prev", x), ("pred_x0", pred_x0)):
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), t.detach().float().cpu().numpy())
     launches = int(lib.vc_launch_count()) + int(unet_m.graph_replayed_launches)   # host-launched + executed through graph replays
     t_dev = torch.tensor([e0.elapsed_time(e1) * 1e-3], device=device, dtype=torch.float64)
     finite = bool(torch.isfinite(x).all())

@@ -1,4 +1,4 @@
-/* vc_b200.h -- C ABI of libvc_b200.so: the sm_100a kernels behind ViewCrafter's DDIM-denoise hot path.
+/* vc_b200.h -- C ABI of libvc_b200.so: the sm_90a kernels behind ViewCrafter's DDIM-denoise hot path.
  *
  * Boundary contract (SURVEY.md 8b): the reference has no FFI of its own on this path -- its "plugin API" is the
  * Python class surface (DDIMSampler.sample / UNetModel.forward / AutoencoderKL.decode).  The Python mirror of

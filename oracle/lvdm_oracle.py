@@ -8,7 +8,7 @@ algorithm.  It is device-agnostic: on the CPU it is the checker of the small par
 CUDA device (tensors + state dict moved there, TF32 off -- see ``exact_fp32``) it is the checker
 at the BASELINE.json sizes (25x4x40x64, 25x4x72x128) where a CPU run takes minutes, and, run under
 ``torch.autocast(fp16)`` with ``attention_mode("sdpa")``, it is the stand-in for "the unmodified
-reference in PyTorch eager on the same B200" (viewcrafter.py:98 runs the reference under autocast;
+reference in PyTorch eager on the same GPU" (viewcrafter.py:98 runs the reference under autocast;
 attention.py:175-190 uses xformers' fused attention when present).  Every function cites the reference file:line (paths relative to the upstream
 repo root) it follows.  The block structure is recovered from the *state-dict keys* (which
 are the reference's load-bearing interface, SURVEY.md Appendix B), not from a copy of the

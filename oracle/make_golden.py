@@ -241,13 +241,13 @@ def gen_unet():
         shapes = _load_synth(m, seed=3)
         g = torch.Generator().manual_seed(5)
         x = torch.randn(1, 8, T, H, W, generator=g)
-        ctx = torch.randn(1, 333, 1024, generator=g)
+        ctx = torch.randn(1, 333, 1024, generator=g).half().float()      # fp16-representable: stored exactly as fp16 (file size)
         t = torch.tensor([499])
         fs = torch.tensor([10])
         with torch.no_grad():
             y = m(x, t, context=ctx, fs=fs)
         np.savez_compressed(os.path.join(OUT, f"unet_{name}.npz"), shapes=shapes, kwargs=json.dumps(over),
-                            x=x.numpy(), ctx=ctx.numpy(), t=t.numpy(), fs=fs.numpy(), y=y.numpy())
+                            x=x.numpy(), ctx=ctx.numpy().astype(np.float16), t=t.numpy(), fs=fs.numpy(), y=y.numpy())
         print(name, "out std", float(y.std()), "absmax", float(y.abs().max()))
 
 
@@ -294,9 +294,51 @@ def gen_resampler():
     print("resampler out std", float(y.std()))
 
 
+class _AttrDict(dict):
+    __getattr__ = dict.__getitem__
+
+
+def _attr(x):
+    if isinstance(x, dict):
+        return _AttrDict({k: _attr(v) for k, v in x.items()})
+    if isinstance(x, list):
+        return [_attr(v) for v in x]
+    return x
+
+
+def gen_dropin():
+    """The reference's own VIPLatentDiffusion from its own YAML (reduced widths, toy OpenCLIP towers) run through its own
+    image_guided_synthesis and DDIMSampler(s); the cases, inputs and widths are those of tests/test_dropin_reference_cpu.py."""
+    import copy
+    import yaml
+    from tests import test_dropin_reference_cpu as D
+    ref_shims.install()
+    D._toys()
+    import utils.diffusion_utils as DU
+    import lvdm.models.samplers.ddim as ref_ddim
+    import lvdm.models.samplers.ddim_multiplecond as ref_multi
+
+    def on_cpu(cls):                                      # ddim.py:18-22 hard-codes "cuda"
+        return type("CpuSampler", (cls,), {"register_buffer": lambda self, name, attr: setattr(self, name, attr)})
+
+    DU.DDIMSampler, DU.DDIMSampler_multicond = on_cpu(ref_ddim.DDIMSampler), on_cpu(ref_multi.DDIMSampler)
+    cfg = D.reduced_config(yaml.safe_load(open(os.path.join(ref_shims.REF_ROOT, "configs", "inference_pvd_1024.yaml")))["model"])
+    for multi, T in D.CASES:
+        torch.manual_seed(0)
+        ref = DU.instantiate_from_config(_attr(copy.deepcopy(cfg))).eval()
+        shapes = [(n, s) for n, s in synth.module_shapes(ref) if n.startswith(D.DROPIN_PREFIXES)]
+        ref.load_state_dict(synth.synth_state_dict(shapes, seed=D.SD_SEED), strict=False)
+        videos, noise_shape, kw = D.inputs(multi, T)
+        torch.manual_seed(11)
+        out = DU.image_guided_synthesis(ref, ["a photo"], videos, noise_shape, **kw)
+        np.savez_compressed(os.path.join(OUT, D.golden_name(multi, T)), config=json.dumps(cfg), shapes=json.dumps([[n, list(s)] for n, s in shapes]),
+                            out=out.numpy().astype(np.float16), out_std=np.float64(out.std()))
+        print("dropin", multi, T, "out std", float(out.std()))
+
+
 if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
-    which = sys.argv[1:] or ["schedule", "ddim", "ddim_options", "ddim_multicond", "unet", "vae", "vae_enc", "resampler"]
+    which = sys.argv[1:] or ["schedule", "ddim", "ddim_options", "ddim_multicond", "unet", "vae", "vae_enc", "resampler", "dropin"]
     with torch.no_grad():
         for w in which:
             globals()["gen_" + w]()

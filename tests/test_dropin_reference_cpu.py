@@ -1,38 +1,56 @@
-"""The drop-in claim, end to end, against the LIVE reference (build container only; skipped where /root/reference is absent):
+"""The drop-in claim, end to end, against outputs of the unmodified reference pipeline (tests/golden/dropin_*.npz).
 
-the reference's own ``VIPLatentDiffusion`` is instantiated from its own YAML (configs/inference_pvd_1024.yaml, reduced widths)
-twice -- once untouched, once with the three ``target:`` lines of INTEGRATION.md pointing at viewcrafter_b200 (UNetModel,
-AutoencoderKL, Resampler) -- the SAME state dict is loaded into both with ``strict=True``, and the reference's own
-``utils.diffusion_utils.image_guided_synthesis`` is run on both (reference DDIMSampler vs viewcrafter_b200 DDIMSampler, the
-one-line import swap of INTEGRATION.md).  The CUDA ops are replaced by the torch double, so this checks every seam of the
-boundary (constructor kwargs, state-dict keys, encode/decode types the reference type-checks, kwargs swallowed by forward, RNG
-order), not the kernels.  Shims: SURVEY.md 8(c) -- a pytorch_lightning stub, an attribute dict for OmegaConf, toy stand-ins for
-the two OpenCLIP towers (open_clip / kornia are not installed), and the CPU register_buffer override of the reference sampler.
-T = 16 so that the per-frame image-token context branch (openaimodel3d.py:556-560) is the one exercised.
+The fixtures were made by oracle/make_golden.py (gen_dropin): the reference's own ``VIPLatentDiffusion``, instantiated from its
+own YAML (configs/inference_pvd_1024.yaml, reduced widths) with synthetic weights, run through the reference's own
+``utils.diffusion_utils.image_guided_synthesis`` and DDIMSampler.  They store the reduced configuration, the (name, shape) list
+of the reference's drop-in sub-modules (``model.diffusion_model``, ``first_stage_model``, ``image_proj_model``) and the output.
+
+Here the same model is assembled from this package alone -- ``LatentDiffusion`` with ``UNetModel``, ``AutoencoderKL`` and
+``Resampler`` built from the reference's constructor kwargs, loaded strictly from the same synthetic state dict under the
+reference's key names -- and ``viewcrafter_b200.synthesis.image_guided_synthesis`` (with ``viewcrafter_b200.ddim``) must
+reproduce the reference output.  The CUDA ops are replaced by the torch double, so this checks every seam of the boundary
+(constructor kwargs, state-dict keys and shapes, conditioning construction, kwargs swallowed by forward, RNG order), not the
+kernels.  The two OpenCLIP towers are toy stand-ins (open_clip / kornia are not installed), identical on both sides.
+T = 16 exercises the per-frame image-token context branch (openaimodel3d.py:556-560), T = 5 the shared-context branch.
 """
-import copy
+import json
+import os
 import sys
 import types
 
+import numpy as np
 import pytest
 import torch
 
-from oracle import ref_shims, synth
+from oracle import synth
 from tests import fake_ops
 
-pytestmark = pytest.mark.skipif(not ref_shims.available(), reason="live reference (/root/reference) not present")
+CASES = [(False, 16), (True, 16), (False, 5)]
+SD_SEED = 81          # synthetic weights of the drop-in sub-modules
+DROPIN_PREFIXES = ("model.diffusion_model.", "first_stage_model.", "image_proj_model.")
 
 
-class _AD(dict):
-    __getattr__ = dict.__getitem__
+def golden_name(multi, T):
+    return f"dropin_{'multicond' if multi else 'cfg'}_T{T}.npz"
 
 
-def _ad(x):
-    if isinstance(x, dict):
-        return _AD({k: _ad(v) for k, v in x.items()})
-    if isinstance(x, list):
-        return [_ad(v) for v in x]
-    return x
+def reduced_config(cfg):
+    """The reference YAML's model section at test widths (mutated in place and returned)."""
+    P = cfg["params"]
+    P["unet_config"]["params"].update(model_channels=64, use_checkpoint=False)
+    P["first_stage_config"]["params"]["ddconfig"].update(ch=32)
+    P["cond_stage_config"] = {"target": "vc_test_toys.ToyText"}
+    P["img_cond_stage_config"] = {"target": "vc_test_toys.ToyImage"}
+    P["image_proj_stage_config"]["params"].update(dim=128, depth=1, heads=2, embedding_dim=64)      # still 16 x 16 queries -> 1024
+    return cfg
+
+
+def inputs(multi, T):
+    H, W = 8, 8
+    videos = torch.rand(1, 3, T, 8 * H, 8 * W, generator=torch.Generator().manual_seed(7)) * 2 - 1
+    kw = dict(n_samples=1, ddim_steps=(1 if multi else 2), ddim_eta=1.0, unconditional_guidance_scale=7.5, cfg_img=(2.0 if multi else None),
+              fs=10, text_input=True, multiple_cond_cfg=multi, timestep_spacing="uniform_trailing", guidance_rescale=0.7, condition_index=[0])
+    return videos, [1, 4, T, H, W], kw
 
 
 def _toys():
@@ -64,72 +82,47 @@ def _toys():
     sys.modules["vc_test_toys"] = m
 
 
-@pytest.mark.parametrize("multi,T", [(False, 16), (True, 16), (False, 5)])
-def test_reference_pipeline_with_dropins_matches_reference(monkeypatch, multi, T):
+def _own_model(P):
+    """VIPLatentDiffusion's surface for image_guided_synthesis, from this package: schedule / scale_arr from the same params,
+    the three drop-in classes from the reference's constructor kwargs, the toy towers as cond_stage_model / embedder."""
+    from viewcrafter_b200.diffusion import LatentDiffusion
+    from viewcrafter_b200.resampler import Resampler
+    m = LatentDiffusion(P["unet_config"]["params"], P["first_stage_config"]["params"], timesteps=P["timesteps"],
+                        linear_start=P["linear_start"], linear_end=P["linear_end"], rescale_betas_zero_snr=P["rescale_betas_zero_snr"],
+                        parameterization=P["parameterization"], scale_factor=P["scale_factor"], use_dynamic_rescale=P["use_dynamic_rescale"],
+                        base_scale=P["base_scale"], perframe_ae=P["perframe_ae"], conditioning_key=P["conditioning_key"])
+    m.image_proj_model = Resampler(**P["image_proj_stage_config"]["params"])
+    toys = sys.modules["vc_test_toys"]
+    m.cond_stage_model, m.embedder = toys.ToyText(), toys.ToyImage()
+    m.get_learned_conditioning = m.cond_stage_model.encode
+    m.uncond_type = P["uncond_type"]
+    return m.eval()
+
+
+@pytest.mark.parametrize("multi,T", CASES)
+def test_reference_pipeline_with_dropins_matches_reference(monkeypatch, golden_dir, multi, T):
     """T = 16: 77 + 16 T = 333 context tokens -> per-frame image tokens (openaimodel3d.py:556-560); T = 5: the shared-context
     branch the 25-frame checkpoints take."""
-    import yaml
-    ref_shims.install()
     _toys()
     fake_ops.install(monkeypatch)
-    import utils.diffusion_utils as DU
-    cfg = yaml.safe_load(open(ref_shims.REF_ROOT + "/configs/inference_pvd_1024.yaml"))["model"]
-    P = cfg["params"]
-    P["unet_config"]["params"].update(model_channels=64, use_checkpoint=False)
-    P["first_stage_config"]["params"]["ddconfig"].update(ch=32)
-    P["cond_stage_config"] = {"target": "vc_test_toys.ToyText"}
-    P["img_cond_stage_config"] = {"target": "vc_test_toys.ToyImage"}
-    P["image_proj_stage_config"]["params"].update(dim=128, depth=1, heads=2, embedding_dim=64)      # still 16 x 16 queries -> 1024
+    z = np.load(os.path.join(golden_dir, golden_name(multi, T)))
+    P = json.loads(str(z["config"]))["params"]
+    ref_shapes = [(n, tuple(s)) for n, s in json.loads(str(z["shapes"]))]
+    mine = _own_model(P)
+    own_shapes = [(k, tuple(v.shape)) for k, v in mine.state_dict().items() if k.startswith(DROPIN_PREFIXES)]
+    assert own_shapes == ref_shapes                       # names, shapes and order of the reference's sub-modules
+    sd = synth.synth_state_dict(ref_shapes, seed=SD_SEED)
+    missing, unexpected = mine.load_state_dict(sd, strict=False)
+    assert not unexpected and all(not k.startswith(DROPIN_PREFIXES) for k in missing)
 
-    def build(ours):
-        c = copy.deepcopy(cfg)
-        if ours:                                          # exactly the YAML edit INTEGRATION.md describes
-            c["params"]["unet_config"]["target"] = "viewcrafter_b200.unet.UNetModel"
-            c["params"]["first_stage_config"]["target"] = "viewcrafter_b200.autoencoder.AutoencoderKL"
-            c["params"]["image_proj_stage_config"]["target"] = "viewcrafter_b200.resampler.Resampler"
-        torch.manual_seed(0)
-        return DU.instantiate_from_config(_ad(c)).eval()
-
-    ref = build(False)
-    sd = synth.synth_state_dict(synth.module_shapes(ref), seed=81)
-    for k, v in ref.state_dict().items():                # schedule buffers keep the values the reference computed
-        if not k.startswith(("model.", "first_stage_model.", "image_proj_model.")):
-            sd[k] = v.clone()
-    ref.load_state_dict(sd, strict=True)
-    mine = build(True)
-    assert list(mine.state_dict().keys()) == list(ref.state_dict().keys())
-    mine.load_state_dict(sd, strict=True)                # load_model_checkpoint(..., strict=True), diffusion_utils.py:83-108
-
-    H, W = 8, 8
-    videos = torch.rand(1, 3, T, 8 * H, 8 * W, generator=torch.Generator().manual_seed(7)) * 2 - 1
-    kw = dict(n_samples=1, ddim_steps=(1 if multi else 2), ddim_eta=1.0, unconditional_guidance_scale=7.5, cfg_img=(2.0 if multi else None),
-              fs=10, text_input=True, multiple_cond_cfg=multi, timestep_spacing="uniform_trailing", guidance_rescale=0.7, condition_index=[0])
-
-    import lvdm.models.samplers.ddim as ref_ddim
-    import lvdm.models.samplers.ddim_multiplecond as ref_multi
-
-    def on_cpu(cls):                                      # ddim.py:18-22 hard-codes "cuda"
-        return type("CpuSampler", (cls,), {"register_buffer": lambda self, name, attr: setattr(self, name, attr)})
-
-    monkeypatch.setattr(DU, "DDIMSampler", on_cpu(ref_ddim.DDIMSampler))
-    monkeypatch.setattr(DU, "DDIMSampler_multicond", on_cpu(ref_multi.DDIMSampler))
-    torch.manual_seed(11)
-    with torch.no_grad():
-        out_ref = DU.image_guided_synthesis(ref, ["a photo"], videos, [1, 4, T, H, W], **kw)
-    from viewcrafter_b200.ddim import DDIMSampler
-    from viewcrafter_b200.ddim_multiplecond import DDIMSampler as DDIMSampler_multicond
-    monkeypatch.setattr(DU, "DDIMSampler", DDIMSampler)                      # the import swap of INTEGRATION.md (b)
-    monkeypatch.setattr(DU, "DDIMSampler_multicond", DDIMSampler_multicond)
-    torch.manual_seed(11)
-    with torch.no_grad():
-        out_mine = DU.image_guided_synthesis(mine, ["a photo"], videos, [1, 4, T, H, W], **kw)
-    assert out_mine.shape == out_ref.shape == (1, 1, 3, T, 8 * H, 8 * W) and out_mine.dtype == out_ref.dtype
-    err = (out_mine - out_ref).abs()
-    std = float(out_ref.std())
-    # fp16 rounding points of the kernels (emulated by the op double) vs the fp32 reference, amplified ~16x by CFG 7.5 per step
-    assert float(err.mean()) < 0.03 * std and float(err.max()) < 0.35 * std, (float(err.mean()), float(err.max()), std)
-    # and our own image_guided_synthesis (viewcrafter_b200/synthesis.py) is the same function on the same model
+    videos, noise_shape, kw = inputs(multi, T)
     from viewcrafter_b200.synthesis import image_guided_synthesis
     torch.manual_seed(11)
-    out_syn = image_guided_synthesis(mine, ["a photo"], videos, [1, 4, T, H, W], **kw)
-    assert float((out_syn - out_mine).abs().mean()) < 0.02 * std
+    with torch.no_grad():
+        out_mine = image_guided_synthesis(mine, ["a photo"], videos, noise_shape, **kw)
+    out_ref = torch.from_numpy(z["out"].astype(np.float32))
+    assert out_mine.shape == out_ref.shape == (1, 1, 3, T, 8 * noise_shape[3], 8 * noise_shape[4]) and out_mine.dtype == torch.float32
+    err = (out_mine - out_ref).abs()
+    std = float(z["out_std"])
+    # fp16 rounding points of the kernels (emulated by the op double) vs the fp32 reference, amplified ~16x by CFG 7.5 per step
+    assert float(err.mean()) < 0.03 * std and float(err.max()) < 0.35 * std, (float(err.mean()), float(err.max()), std)

@@ -36,7 +36,7 @@ def test_unet_wiring_matches_reference_golden(cpu_ops, golden_dir, name):
     kw = dict(UNET_PARAMS); kw.update(json.loads(str(g["kwargs"])))
     m = UNetModel(**kw).eval()
     m.load_state_dict(synth.synth_state_dict(shapes, 3), strict=True)
-    y = m(torch.from_numpy(g["x"]), torch.from_numpy(g["t"]), context=torch.from_numpy(g["ctx"]), fs=torch.from_numpy(g["fs"]))
+    y = m(torch.from_numpy(g["x"]), torch.from_numpy(g["t"]), context=torch.from_numpy(g["ctx"]).float(), fs=torch.from_numpy(g["fs"]))
     err = (y - torch.from_numpy(g["y"])).abs()
     assert float(err.max()) < 0.02 and float(err.mean()) < 0.003, (float(err.max()), float(err.mean()))
 

@@ -1,4 +1,4 @@
-"""Op-level parity of the sm_100a kernels (called through the C ABI) against plain PyTorch fp32 references.
+"""Op-level parity of the sm_90a kernels (called through the C ABI) against plain PyTorch fp32 references.
 
 Tolerances: inputs/outputs are fp16 with fp32 accumulation, so the bound is a few fp16 ulps of the output
 magnitude: |err| <= atol + rtol*|ref| with rtol 4e-3 (fp16 eps = 9.8e-4) unless stated.
@@ -350,40 +350,39 @@ def test_linear_strided_weight_view(ops):
     close(out, ref, 2e-2, rtol=2e-3, what="strided w")
 
 
-def test_gemm_cta_pair_path(ops):
-    """Shapes large enough to be routed to the tcgen05 cta_group::2 kernel (>= 148 tile pairs): odd m-tile counts
-    (last pair half empty), ragged M, bias + residual, GEGLU, K-split concat, 3x3 conv taps and temporal taps."""
+def test_gemm_many_tile_rounds(ops):
+    """Large shapes (more tiles than SMs, several persistent rounds): odd m-tile counts, ragged M, bias + residual, GEGLU, K-split concat, 3x3 conv taps and temporal taps."""
     M = 128 * 301 + 37
     x, w = rnd(M, 320, seed=80), rnd(320, 320, seed=81, scale=320 ** -0.5)
     b, r = rnd(320, seed=82, dtype=torch.float32), rnd(M, 320, seed=83)
-    close(ops.linear(x, w, bias=b, res=r), x.float() @ w.float().t() + b + r.float(), 4e-3, what="pair linear 160")
+    close(ops.linear(x, w, bias=b, res=r), x.float() @ w.float().t() + b + r.float(), 4e-3, what="many-tile linear N=320")
     w2 = rnd(1024, 320, seed=84, scale=320 ** -0.5)
-    close(ops.linear(x, w2), x.float() @ w2.float().t(), 2e-3, what="pair linear 256")
+    close(ops.linear(x, w2), x.float() @ w2.float().t(), 2e-3, what="many-tile linear N=1024")
     wg = rnd(2560, 320, seed=85, scale=320 ** -0.5)
     bg = rnd(2560, seed=86, dtype=torch.float32, scale=0.1)
     hh = x.float() @ wg.float().t() + bg
     wp, bp = ops.pack_geglu(wg, bg)
-    close(ops.linear(x, wp, bias=bp, geglu=True), hh[:, :1280] * F.gelu(hh[:, 1280:]), 4e-3, what="pair geglu")
+    close(ops.linear(x, wp, bias=bp, geglu=True), hh[:, :1280] * F.gelu(hh[:, 1280:]), 4e-3, what="many-tile geglu")
     a2 = rnd(M, 128, seed=87)
     w3 = rnd(384, 448, seed=88, scale=448 ** -0.5)
-    close(ops.linear(x, w3, x2=a2), torch.cat([x, a2], 1).float() @ w3.float().t(), 2e-3, what="pair concat-K")
+    close(ops.linear(x, w3, x2=a2), torch.cat([x, a2], 1).float() @ w3.float().t(), 2e-3, what="many-tile concat-K")
     frames, H, W, Ci, Co = 5, 72, 128, 64, 256
     xi = rnd(frames, Ci, H, W, seed=89)
     wc = rnd(Co, Ci, 3, 3, seed=90, scale=(9 * Ci) ** -0.5)
     bc = rnd(Co, seed=91, dtype=torch.float32)
     ref = _nhwc_rows(F.conv2d(xi.float(), wc.float(), bc, padding=1))
-    close(ops.conv3x3(_nhwc_rows(xi), frames, H, W, ops.pack_conv3x3(wc), bias=bc), ref, 3e-3, what="pair conv3x3")
+    close(ops.conv3x3(_nhwc_rows(xi), frames, H, W, ops.pack_conv3x3(wc), bias=bc), ref, 3e-3, what="many-tile conv3x3")
     frames, H, W, Ci, Co = 41, 18, 32, 64, 128                     # 5 tiles per frame (last one ragged), odd tile count
     xi = rnd(frames, Ci, H, W, seed=92)
     wc = rnd(Co, Ci, 3, 3, seed=93, scale=(9 * Ci) ** -0.5)
     ref = _nhwc_rows(F.conv2d(xi.float(), wc.float(), None, padding=1))
-    close(ops.conv3x3(_nhwc_rows(xi), frames, H, W, ops.pack_conv3x3(wc)), ref, 3e-3, what="pair conv3x3 ragged")
+    close(ops.conv3x3(_nhwc_rows(xi), frames, H, W, ops.pack_conv3x3(wc)), ref, 3e-3, what="many-tile conv3x3 ragged")
     B, T, HW, C = 1, 5, 9216, 128
     x5 = rnd(B, C, T, HW, 1, seed=94)
     wt = rnd(C, C, 3, 1, 1, seed=95, scale=(3 * C) ** -0.5)
     ref5 = F.conv3d(x5.float(), wt.float(), None, padding=(1, 0, 0))
     rows = lambda t5: t5.permute(0, 2, 3, 4, 1).reshape(B * T * HW, C).contiguous()
-    close(ops.conv_temporal(rows(x5), B, T, HW, ops.pack_conv_temporal(wt)), rows(ref5), 3e-3, what="pair conv_temporal")
+    close(ops.conv_temporal(rows(x5), B, T, HW, ops.pack_conv_temporal(wt)), rows(ref5), 3e-3, what="many-tile conv_temporal")
 
 
 def test_softmax_rows(ops):
@@ -424,7 +423,7 @@ def test_upsample_conv_fused(ops, frames, H, W, Ci, Co):
 
 @pytest.mark.parametrize("env", [{"VC_ATTN_BN64": "0"}, {"VC_ATTN_BN64": "1"}])
 def test_attention_kernel_variants(env):
-    """Both attention kernels (128-key tiles, two CTAs per SM / 64-key tiles, three CTAs per SM), forced for ALL shapes through the environment in a
+    """Both attention tile widths (128-key tiles, one CTA per SM / 64-key tiles, two CTAs per SM), forced for ALL shapes through the environment in a
     fresh process (the choice is cached per process), against the fp32 reference: tools/attn_check.py."""
     import os, subprocess, sys
     if not torch.cuda.is_available():
@@ -524,8 +523,8 @@ def test_groupnorm_concat_from_partial_sums(ops, monkeypatch, C1, C2):
     close(ops.groupnorm(a2, frames, g, b, 1e-5, True, x2=s), ref, 3e-3, what="concat fallback")
 
 
-def test_gemm_output_unchanged_by_gn_out_cta_pair_and_single(ops, monkeypatch):
-    """Large problems run on CTA pairs (m-tile count padded to even), small ones on single CTAs: records of both kernels are consumed."""
+def test_gemm_output_unchanged_by_gn_out_large_and_small(ops, monkeypatch):
+    """Large and small tile counts (several persistent rounds / fewer tiles than SMs): the records of both are consumed."""
     _force_gn_parts(ops, monkeypatch)
     for M, K, N in ((128 * 301, 320, 320), (128 * 3 + 40, 640, 640), (40000, 1280, 320)):
         x, w = rnd(M, K, seed=91), rnd(N, K, seed=92, scale=2.0 * K ** -0.5)

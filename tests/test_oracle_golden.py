@@ -79,7 +79,7 @@ def test_unet_matches_reference(golden_dir, name):
     shapes = [(n, tuple(s)) for n, s in json.loads(str(g["shapes"]))]
     sd = synth.synth_state_dict(shapes, seed=3)
     with torch.no_grad():
-        y = O.unet_forward(sd, torch.from_numpy(g["x"]), torch.from_numpy(g["t"]), torch.from_numpy(g["ctx"]),
+        y = O.unet_forward(sd, torch.from_numpy(g["x"]), torch.from_numpy(g["t"]), torch.from_numpy(g["ctx"]).float(),
                            torch.from_numpy(g["fs"]))
     np.testing.assert_allclose(y.numpy(), g["y"], rtol=0, atol=5e-5)
 

@@ -44,14 +44,15 @@ for name, H, W, C in (("l0", 72, 128, 320), ("l1", 36, 64, 640), ("l2", 18, 32, 
         by = 2.0 * M * C * 2
         print(f"[gn-parts] {name} C={C:4d} groupnorm {cn}: statistics pass {ta*1e6:8.1f} us ({by/ta/1e9:6.0f} GB/s)   from producer sums {tb*1e6:8.1f} us "
               f"({by/tb/1e9:6.0f} GB/s r+w once)   |diff| {err:.2e}")
-# B = 2 (what a CFG step runs): 50 frames at level 0
-M = 2 * T * 72 * 128
-x = (torch.randn(M, 320, device="cuda") * 0.8).half()
-w9 = (torch.randn(9 * 320, 320, device="cuda") * 0.02).half()
-g, b = torch.rand(320, device="cuda") + 0.5, torch.randn(320, device="cuda") * 0.1
-y = ops.conv3x3(x, 2 * T, 72, 128, w9, gn_out=True)
-yc = y.clone()
-for cn, samples in (("4-D B=2", 2 * T), ("5-D B=2", 2)):
-    ta, tb = t(lambda: ops.groupnorm(yc, samples, g, b, 1e-5, True)), t(lambda: ops.groupnorm(y, samples, g, b, 1e-5, True))
-    by = 2.0 * M * 320 * 2
-    print(f"[gn-parts] l0 C= 320 groupnorm {cn}: statistics pass {ta*1e6:8.1f} us ({by/ta/1e9:6.0f} GB/s)   from producer sums {tb*1e6:8.1f} us ({by/tb/1e9:6.0f} GB/s r+w once)")
+# B = 2 (what a CFG step runs): per-frame GroupNorm over 50 frames at every level -- the tensor sizes ops.GN_PARTS_MIN_MB chooses between
+for name, H, W, C in (("l0", 72, 128, 320), ("l1", 36, 64, 640), ("l2", 18, 32, 1280), ("l3", 9, 16, 1280)):
+    M = 2 * T * H * W
+    x = (torch.randn(M, C, device="cuda") * 0.8).half()
+    w9 = (torch.randn(9 * C, C, device="cuda") * (1.0 / (3 * C ** 0.5))).half()
+    g, b = torch.rand(C, device="cuda") + 0.5, torch.randn(C, device="cuda") * 0.1
+    y = ops.conv3x3(x, 2 * T, H, W, w9, gn_out=True)
+    yc = y.clone()
+    for cn, samples in (("4-D B=2", 2 * T), ("5-D B=2", 2)):
+        ta, tb = t(lambda: ops.groupnorm(yc, samples, g, b, 1e-5, True)), t(lambda: ops.groupnorm(y, samples, g, b, 1e-5, True))
+        by = 2.0 * M * C * 2
+        print(f"[gn-parts] {name} C={C:4d} {M * C * 2 / 1e6:6.0f} MB groupnorm {cn}: statistics pass {ta*1e6:8.1f} us   from producer sums {tb*1e6:8.1f} us")

@@ -1,4 +1,4 @@
-"""viewcrafter_b200: B200-native (sm_100a) implementation of ViewCrafter's DDIM-denoise hot path.
+"""viewcrafter_b200: H100-native (sm_90a) implementation of ViewCrafter's DDIM-denoise hot path.
 
 Drop-in classes (same names / constructor kwargs / state-dict keys as the reference):
     viewcrafter_b200.unet.UNetModel             <- lvdm.modules.networks.openaimodel3d.UNetModel
@@ -7,6 +7,6 @@ Drop-in classes (same names / constructor kwargs / state-dict keys as the refere
     viewcrafter_b200.ddim_multiplecond.DDIMSampler <- lvdm.models.samplers.ddim_multiplecond.DDIMSampler
     viewcrafter_b200.resampler.Resampler        <- lvdm.modules.encoders.resampler.Resampler
     viewcrafter_b200.synthesis.image_guided_synthesis / get_latent_z <- utils.diffusion_utils (same names)
-All tensor work runs in libvc_b200.so (hand-written CUDA for sm_100a, C ABI in include/vc_b200.h).
+All tensor work runs in libvc_b200.so (hand-written CUDA for sm_90a, C ABI in include/vc_b200.h).
 """
 __version__ = "0.1.0"

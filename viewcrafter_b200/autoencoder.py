@@ -1,8 +1,8 @@
 """Drop-in ``AutoencoderKL`` (reference: lvdm/models/autoencoder.py:13-107, lvdm/modules/networks/ae_modules.py).
 
-``decode(z)`` -- the hot-path half -- runs on the sm_100a kernels: post_quant 1x1 GEMM, conv_in, ResnetBlocks
-(GroupNorm+swish kernel, 9-tap tcgen05 GEMMs, 1x1 nin_shortcut fused as residual), the single-head d=512 AttnBlock
-(QK^T and PV as tcgen05 GEMMs around a row-softmax kernel), nearest-2x upsample + conv, GroupNorm+swish, conv_out.
+``decode(z)`` -- the hot-path half -- runs on the sm_90a kernels: post_quant 1x1 GEMM, conv_in, ResnetBlocks
+(GroupNorm+swish kernel, 9-tap wgmma GEMMs, 1x1 nin_shortcut fused as residual), the single-head d=512 AttnBlock
+(QK^T and PV as wgmma GEMMs around a row-softmax kernel), nearest-2x upsample + conv, GroupNorm+swish, conv_out.
 State-dict keys match the reference (``post_quant_conv.*``, ``decoder.*``, ``encoder.*``, ``quant_conv.*``).
 ``encode(x)`` (conditioning renders, once per clip; SURVEY.md 8f rank f1) runs the Encoder on the same kernels: the stride-2
 Downsample (zero-pad right/bottom, ae_modules.py:102-106) is an im2col + GEMM, and conv_out is folded with the 1x1 quant_conv;

@@ -1,26 +1,20 @@
-// FlashAttention-style fused softmax(Q K^T * scale) V for head_dim 64 on tcgen05 (sm_100a).
+// FlashAttention-style fused softmax(Q K^T * scale) V for head_dim 64 on wgmma (sm_90a).
 //
 // Used for the spatial self-attention (Nq = Nk = H*W up to 9216) and the text / image cross-attention
-// (Nk = 77 / 256) of lvdm/modules/attention.py:81-144.  One CTA owns 128 query rows of one (batch, head)
-// and streams 128-key tiles:
-//     S = Q K^T          SS MMA, fp32 accumulator in TMEM
-//     online softmax     128 threads, one query row each: the whole 128-wide S row is pulled into registers with
-//                        four back-to-back tcgen05.ld and ONE wait; exp2 domain; the running maximum is only
-//                        refreshed when it grew by more than 2^8 ("lazy rescale"), so O is rarely touched
-//     P (fp16) -> TMEM, O += P V   TS MMA (A from TMEM, V tile MN-major in smem)
-// The next tile's Q K^T is issued as soon as S sits in registers, so the tensor pipe works underneath the
-// MUFU-bound softmax; K and V tiles arrive by TMA through two separate 2-stage mbarrier rings: a K stage is released as
-// soon as its Q K^T has retired, a V stage when its P V has, so K(j+1) is in flight a whole tile period before
-// Q K^T(j+1) is issued (with one shared K/V ring the load could only start when P V(j-1) had retired, i.e. exactly when
-// it was needed: ncu showed the softmax warps waiting for S 9 % of the time).  Two CTAs are co-resident per SM.
-//
-// Warp roles (192 threads): warp0 = TMA producer, warp1 = TMEM alloc + MMA issuer, warps2..5 = softmax /
-// correction / epilogue (TMEM lane quadrant = warp % 4).
-// TMEM columns: [0,128) S fp32 | [128,192) P fp16x2 | [192,256) O fp32.
+// (Nk = 77 / 256) of lvdm/modules/attention.py:81-144.  One CTA owns 128 query rows of one (batch, head) and streams
+// BNK-key tiles of K and V through a two-stage TMA ring.  Each of the two MMA warpgroups owns 64 query rows:
+//     S = Q K^T          wgmma m64nBNKk16, both operands from shared memory (128B-swizzled TMA tiles)
+//     online softmax     on the accumulator fragments (two rows per thread, row max / sum over the 4-lane quad), exp2 domain
+//     O += P V           wgmma with P as the register A operand (the S fragments re-packed to fp16 in place) and the V tile
+//                        read MN-major (tnspB) straight from the TMA tile
+// Warp roles (288 threads): warps 0..7 = two MMA / softmax warpgroups, warp 8 = TMA producer.
+// Two tile widths: 64 keys (short key sequences: cross-attention, the 18x32 and 9x16 levels; smaller register and
+// shared-memory footprint, two CTAs per SM) and 128 keys (long sequences: half the barrier round trips per key).
 #include <cstdlib>
 
 #include "common.cuh"
 #include "kernels.h"
+#include "wgmma.cuh"
 
 namespace vc {
 
@@ -34,382 +28,184 @@ struct AttnParams {
   int accumulate;
 };
 
-static constexpr int ATT_BM = 128, ATT_BN = 128, ATT_D = 64;
-static constexpr int ATT_TILE_BYTES = 128 * 64 * 2;                    // 16 KB
-static constexpr int ATT_SMEM = ATT_TILE_BYTES * 5 + 1024 + 256;       // Q + 2x(K,V) + slack + barriers
-static constexpr float ATT_LAZY = 8.0f;                                // rescale only if the max grew by > 2^8
-// A/B switches (side-by-side builds: VC_NVCC_EXTRA="-DVC_ATT_SPLIT_KV=0 ..." + VC_OUT, loaded through VC_B200_LIB)
-#ifndef VC_ATT_SPLIT_KV
-#define VC_ATT_SPLIT_KV 1      // separate K / V rings (0: one ring, a stage is freed when its P V retires)
-#endif
-#ifndef VC_ATT_PARKED_WAIT
-#define VC_ATT_PARKED_WAIT 0   // TMA / MMA warps wait through try_wait with a suspend-time hint instead of spinning (measured 3 % slower)
-#endif
-#if VC_ATT_PARKED_WAIT
-#define ATT_ROLE_WAIT mbar_wait_parked
-#else
-#define ATT_ROLE_WAIT mbar_wait
-#endif
+static constexpr int ATT_BM = 128, ATT_D = 64;
+static constexpr int ATT_THREADS = 288;
+static constexpr int ATT_Q_BYTES = ATT_BM * ATT_D * 2;                 // 16 KB
+
+template <int BNK>
+struct AttnCfg {
+  static constexpr int KV_BYTES = BNK * ATT_D * 2;
+  static constexpr int SMEM = ATT_Q_BYTES + 4 * KV_BYTES + 1024 + 256;  // Q + 2 x (K, V) + alignment slack + barriers
+  static constexpr int MIN_CTAS = BNK == 64 ? 2 : 1;
+};
 
 __device__ __forceinline__ float ex2f(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// exp2 on the FMA/ALU pipes (Cody-Waite split + degree-3 minimax polynomial, rel. error 1.0e-4, below the 4.9e-4 fp16 resolution of P):
-// the MUFU pipe is the binding unit of d=64 attention (ncu: XU 72.7 % vs tensor 35.7 %), so one probability in every
-// ATT_POLY_PERIOD is computed here instead.
-__device__ __forceinline__ float ex2_poly(float x) {
-  x = fmaxf(x, -125.0f);
-  const float xf = x + 12582912.0f;                       // 1.5 * 2^23: integer part lands in the low mantissa bits
-  const float f = x - (xf - 12582912.0f);                 // f in [-0.5, 0.5]
-  float p = fmaf(f, 0.05592204f, 0.24264008f);          // Chebyshev-node fit of 2^f on [-0.5, 0.5]: max rel. error 1.03e-4
-  p = fmaf(p, f, 0.69312102f);
-  p = fmaf(p, f, 0.99992448f);
-  return __int_as_float(__float_as_int(p) + (__float_as_int(xf) << 23));
-}
-#ifndef VC_ATT_POLY_PERIOD
-#define VC_ATT_POLY_PERIOD 4
-#endif
-static constexpr int ATT_POLY_PERIOD = VC_ATT_POLY_PERIOD;   // one pair in every PERIOD pairs on the FMA pipe; 0 disables the polynomial path
-__device__ __forceinline__ float ex2_sel(float x, int e) {
-  if (ATT_POLY_PERIOD > 0 && (e % (2 * ATT_POLY_PERIOD)) < 2) return ex2_poly(x);
-  return ex2f(x);
-}
 
-#ifndef VC_ATT_F32X2
-#define VC_ATT_F32X2 1
-#endif
-// two exponentials at once: both on MUFU, or (one pair in every ATT_POLY_PERIOD) both through the polynomial in packed fp32x2
-#ifndef VC_ATT_POLY_SEL
-#define VC_ATT_POLY_SEL(e) (ATT_POLY_PERIOD > 0 && ((e) % (2 * ATT_POLY_PERIOD)) < 2)     // which pairs of a 32-score chunk take the polynomial
-#endif
-__device__ __forceinline__ float2 ex2_pair(float2 x, int e) {
-  if (VC_ATT_POLY_SEL(e)) {
-    x.x = fmaxf(x.x, -125.0f);
-    x.y = fmaxf(x.y, -125.0f);
-    const float2 magic = make_float2(12582912.0f, 12582912.0f), nmagic = make_float2(-12582912.0f, -12582912.0f);
-    const float2 xf = __fadd2_rn(x, magic);                                   // integer part in the low mantissa bits
-    const float2 t = __fadd2_rn(xf, nmagic);
-    const float2 f = __ffma2_rn(t, make_float2(-1.f, -1.f), x);               // f in [-0.5, 0.5]
-    float2 p = __ffma2_rn(f, make_float2(0.05592204f, 0.05592204f), make_float2(0.24264008f, 0.24264008f));
-    p = __ffma2_rn(p, f, make_float2(0.69312102f, 0.69312102f));
-    p = __ffma2_rn(p, f, make_float2(0.99992448f, 0.99992448f));
-    float2 r;
-    r.x = __int_as_float(__float_as_int(p.x) + (__float_as_int(xf.x) << 23));
-    r.y = __int_as_float(__float_as_int(p.y) + (__float_as_int(xf.y) << 23));
-    return r;
-  }
-  return make_float2(ex2f(x.x), ex2f(x.y));
-}
-
-__global__ void __launch_bounds__(192, 2) flash_attn_d64_kernel(const __grid_constant__ AttnParams p) {
+template <int BNK>
+__global__ void __launch_bounds__(ATT_THREADS, AttnCfg<BNK>::MIN_CTAS) flash_attn_d64_kernel(const __grid_constant__ AttnParams p) {
+  using Cfg = AttnCfg<BNK>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;
-  uint8_t* sKV = smem + ATT_TILE_BYTES;                                 // stage s: K at s*32K, V at s*32K+16K
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 5 * ATT_TILE_BYTES);
+  uint8_t* sKV = smem + ATT_Q_BYTES;                                    // stage s: K at s * 2 KV, V at s * 2 KV + KV
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + ATT_Q_BYTES + 4 * Cfg::KV_BYTES);
   uint64_t* q_full = bars + 0;
-  uint64_t* kv_full = bars + 1;    // [2]  K tile landed (one-ring build: K and V)
-  uint64_t* kv_empty = bars + 3;   // [2]  K stage free: its Q K^T retired (one-ring build: its P V retired)
-  uint64_t* s_full = bars + 5;     // MMA -> softmax: S tile ready
-  uint64_t* s_free = bars + 6;     // softmax -> MMA: S tile copied to registers (one arrival per softmax warp)
-  uint64_t* p_full = bars + 7;     // softmax -> MMA: P written, O corrected (one arrival per softmax warp)
-  uint64_t* o_done = bars + 8;     // MMA -> softmax: P V of the tile retired
-  uint64_t* v_full = bars + 9;     // [2]  V tile landed
-  uint64_t* v_empty = bars + 11;   // [2]  V stage free: its P V retired
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 13);
+  uint64_t* kv_full = bars + 1;    // [2]  K and V tiles landed
+  uint64_t* kv_empty = bars + 3;   // [2]  both warpgroups are done with the stage (one arrival per MMA warp)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * ATT_BM, head = blockIdx.y, b = blockIdx.z;
   const int bk = p.kv_shared ? 0 : b;
-  const int ntiles = (p.Nk + ATT_BN - 1) / ATT_BN;
+  const int ntiles = (p.Nk + BNK - 1) / BNK;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.tmap_q);
     tma_prefetch_desc(&p.tmap_k);
     tma_prefetch_desc(&p.tmap_v);
     mbar_init(q_full, 1);
     mbar_init(&kv_full[0], 1); mbar_init(&kv_full[1], 1);
-    mbar_init(&kv_empty[0], 1); mbar_init(&kv_empty[1], 1);
-    mbar_init(&v_full[0], 1); mbar_init(&v_full[1], 1);
-    mbar_init(&v_empty[0], 1); mbar_init(&v_empty[1], 1);
-    mbar_init(s_full, 1);
-    mbar_init(s_free, 4);      // one arrival per softmax warp (512 serialised mbarrier arrivals per tile were measurable)
-    mbar_init(p_full, 4);
-    mbar_init(o_done, 1);
+    mbar_init(&kv_empty[0], 8); mbar_init(&kv_empty[1], 8);
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 256);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tS = tmem_base, tP = tmem_base + 128, tO = tmem_base + 192;
 
-  // warps 0/1 run warp-uniform loops and ONE elected lane issues TMA / MMA (keeps operands in uniform registers)
-  if (warp == 0) {
+  if (warp == 8) {
+    // ------------------------------ TMA producer ------------------------------
     if (elect_one()) {
-      mbar_expect_tx(q_full, ATT_TILE_BYTES);
+      mbar_expect_tx(q_full, ATT_Q_BYTES);
       tma_load_4d(sQ, &p.tmap_q, q_full, 0, head, q0, b);
     }
     __syncwarp();
     for (int j = 0; j < ntiles; ++j) {
       const int s = j & 1;
-      uint8_t* sk = sKV + s * 2 * ATT_TILE_BYTES;
-#if VC_ATT_SPLIT_KV
-      if (j >= 2) ATT_ROLE_WAIT(&kv_empty[s], ((j >> 1) - 1) & 1);        // Q K^T(j-2) retired
+      uint8_t* sk = sKV + s * 2 * Cfg::KV_BYTES;
+      if (j >= 2) mbar_wait(&kv_empty[s], ((j >> 1) - 1) & 1);          // tile j-2 fully consumed
       if (elect_one()) {
-        mbar_expect_tx(&kv_full[s], ATT_TILE_BYTES);
-        tma_load_4d(sk, &p.tmap_k, &kv_full[s], 0, head, j * ATT_BN, bk);
-      }
-      __syncwarp();
-      if (j >= 2) ATT_ROLE_WAIT(&v_empty[s], ((j >> 1) - 1) & 1);         // P V(j-2) retired
-      if (elect_one()) {
-        mbar_expect_tx(&v_full[s], ATT_TILE_BYTES);
-        tma_load_4d(sk + ATT_TILE_BYTES, &p.tmap_v, &v_full[s], 0, head, j * ATT_BN, bk);
-      }
-      __syncwarp();
-#else
-      if (j >= 2) ATT_ROLE_WAIT(&kv_empty[s], ((j >> 1) - 1) & 1);
-      if (elect_one()) {
-        mbar_expect_tx(&kv_full[s], 2 * ATT_TILE_BYTES);
-        tma_load_4d(sk, &p.tmap_k, &kv_full[s], 0, head, j * ATT_BN, bk);
-        tma_load_4d(sk + ATT_TILE_BYTES, &p.tmap_v, &kv_full[s], 0, head, j * ATT_BN, bk);
-      }
-      __syncwarp();
-#endif
-    }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc_qk = umma_idesc_f16(128, 128, 0, 0);
-    constexpr uint32_t idesc_pv = umma_idesc_f16(128, 64, 0, 1);      // B = V is MN-major
-    const uint32_t aQ = smem_u32(sQ);
-    auto issue_qk = [&](int j) {
-      const int s = j & 1;
-      ATT_ROLE_WAIT(&kv_full[s], (j >> 1) & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t aK = smem_u32(sKV + s * 2 * ATT_TILE_BYTES);
-#pragma unroll
-        for (int k = 0; k < ATT_D / 16; ++k)
-          umma_ss(tS, umma_desc_sw128(aQ + k * 32), umma_desc_sw128(aK + k * 32), idesc_qk, k > 0 ? 1u : 0u);
-        umma_commit(s_full);
-#if VC_ATT_SPLIT_KV
-        umma_commit(&kv_empty[s]);                // the K stage is free once this Q K^T has retired
-#endif
-      }
-      __syncwarp();
-    };
-    ATT_ROLE_WAIT(q_full, 0);
-    issue_qk(0);
-    for (int j = 0; j < ntiles; ++j) {
-      if (j + 1 < ntiles) {                       // next S as soon as this one has been copied out of TMEM
-        ATT_ROLE_WAIT(s_free, j & 1);
-        issue_qk(j + 1);
-      }
-#if VC_ATT_SPLIT_KV
-      ATT_ROLE_WAIT(&v_full[j & 1], (j >> 1) & 1);
-#endif
-      ATT_ROLE_WAIT(p_full, j & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t aV = smem_u32(sKV + (j & 1) * 2 * ATT_TILE_BYTES) + ATT_TILE_BYTES;
-#pragma unroll
-        for (int k = 0; k < ATT_BN / 16; ++k)
-          umma_ts(tO, tP + k * 8, umma_desc_sw128(aV + k * 2048), idesc_pv, (j > 0 || k > 0) ? 1u : 0u);
-#if VC_ATT_SPLIT_KV
-        umma_commit(&v_empty[j & 1]);
-#else
-        umma_commit(&kv_empty[j & 1]);
-#endif
-        umma_commit(o_done);
+        mbar_expect_tx(&kv_full[s], 2 * Cfg::KV_BYTES);
+        tma_load_4d(sk, &p.tmap_k, &kv_full[s], 0, head, j * BNK, bk);
+        tma_load_4d(sk + Cfg::KV_BYTES, &p.tmap_v, &kv_full[s], 0, head, j * BNK, bk);
       }
       __syncwarp();
     }
-  } else {
-    const int qd = warp & 3;
-    const int r = qd * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(qd * 32) << 16;
-    const float sl2 = p.scale_log2;
-    float m = -INFINITY, l = 0.f;
-    for (int j = 0; j < ntiles; ++j) {
-      const int valid = min(ATT_BN, p.Nk - j * ATT_BN);
-      mbar_wait(s_full, j & 1);
-      tc_fence_after();
-      uint32_t s0[32], s1[32], s2[32], s3[32];
-      tmem_ld32(tS + lane_off, s0);
-      tmem_ld32(tS + lane_off + 32, s1);
-      tmem_ld32(tS + lane_off + 64, s2);
-      tmem_ld32(tS + lane_off + 96, s3);
-      tc_wait_ld();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_relaxed(s_free);
-
-      float mx = -INFINITY;
-      if (valid == ATT_BN) {
-        // four independent running maxima (one per 32-column chunk): a single chain is 32 dependent FMNMX deep
-        float m0 = -INFINITY, m1 = -INFINITY, m2 = -INFINITY, m3 = -INFINITY;
-#pragma unroll
-        for (int e = 0; e < 32; e += 2) {
-          m0 = fmaxf(m0, fmaxf(__uint_as_float(s0[e]), __uint_as_float(s0[e + 1])));
-          m1 = fmaxf(m1, fmaxf(__uint_as_float(s1[e]), __uint_as_float(s1[e + 1])));
-          m2 = fmaxf(m2, fmaxf(__uint_as_float(s2[e]), __uint_as_float(s2[e + 1])));
-          m3 = fmaxf(m3, fmaxf(__uint_as_float(s3[e]), __uint_as_float(s3[e + 1])));
-        }
-        mx = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3));
-      } else {
-#pragma unroll
-        for (int e = 0; e < 32; ++e) {
-          if (e >= valid) s0[e] = 0xff800000u;            // -inf: masked keys get probability 0
-          if (32 + e >= valid) s1[e] = 0xff800000u;
-          if (64 + e >= valid) s2[e] = 0xff800000u;
-          if (96 + e >= valid) s3[e] = 0xff800000u;
-          mx = fmaxf(mx, fmaxf(fmaxf(__uint_as_float(s0[e]), __uint_as_float(s1[e])), fmaxf(__uint_as_float(s2[e]), __uint_as_float(s3[e]))));
-        }
-      }
-      const float m_cand = fmaxf(m, mx * sl2);
-      const bool need = (m_cand - m) > ATT_LAZY;          // j == 0: m = -inf -> true
-      float alpha = 1.f;
-      if (need) {
-        alpha = ex2f(m - m_cand);                         // 0 at j == 0
-        l *= alpha;
-        m = m_cand;
-      }
-      const float neg_m = -m;
-#if VC_ATT_F32X2
-      // packed fp32x2 arithmetic (FFMA2 / FADD2, sm_100): the softmax warps are issue-slot bound (ncu round 1: 7.9 warp
-      // instructions per 32 scores, issue slots 65 % busy, tensor pipe 36 %), and the scale-subtract, the row sums and the
-      // polynomial exp2 are all two-at-a-time.  Per score: 0.5 FFMA2 + 1 MUFU (or the polynomial) + 0.5 FADD2 + 0.5 F2FP.
-      const float2 sl2v = make_float2(sl2, sl2), negm2 = make_float2(neg_m, neg_m);
-      float2 ps0 = make_float2(0.f, 0.f), ps1 = ps0, ps2 = ps0, ps3 = ps0;
-#define VC_ATT_CHUNK(SRC, DST, OFF, PS)                                                                       \
-  _Pragma("unroll") for (int e = 0; e < 32; e += 2) {                                                         \
-    const float2 x = __ffma2_rn(make_float2(__uint_as_float(SRC[e]), __uint_as_float(SRC[e + 1])), sl2v, negm2); \
-    const float2 a = ex2_pair(x, e);                                                                          \
-    PS = __fadd2_rn(PS, a);                                                                                   \
-    DST[OFF + e / 2] = pack_half2(a.x, a.y);                                                                  \
-  }
-      VC_ATT_CHUNK(s0, s0, 0, ps0)
-      VC_ATT_CHUNK(s1, s0, 16, ps1)
-      VC_ATT_CHUNK(s2, s2, 0, ps2)
-      VC_ATT_CHUNK(s3, s2, 16, ps3)
-#undef VC_ATT_CHUNK
-      const float2 pst = __fadd2_rn(__fadd2_rn(ps0, ps1), __fadd2_rn(ps2, ps3));
-      l += pst.x + pst.y;
-#else
-      float ps0 = 0.f, ps1 = 0.f, ps2 = 0.f, ps3 = 0.f;     // independent partial row sums (shorter FADD chains)
-      // probabilities, packed in place: s0[0..15] <- s0, s0[16..31] <- s1, s2[0..15] <- s2, s2[16..31] <- s3
-#pragma unroll
-      for (int e = 0; e < 32; e += 2) {
-        const float a0 = ex2_sel(fmaf(__uint_as_float(s0[e]), sl2, neg_m), e), a1 = ex2_sel(fmaf(__uint_as_float(s0[e + 1]), sl2, neg_m), e + 1);
-        ps0 += a0 + a1;
-        s0[e / 2] = pack_half2(a0, a1);
-      }
-#pragma unroll
-      for (int e = 0; e < 32; e += 2) {
-        const float a0 = ex2_sel(fmaf(__uint_as_float(s1[e]), sl2, neg_m), e), a1 = ex2_sel(fmaf(__uint_as_float(s1[e + 1]), sl2, neg_m), e + 1);
-        ps1 += a0 + a1;
-        s0[16 + e / 2] = pack_half2(a0, a1);
-      }
-#pragma unroll
-      for (int e = 0; e < 32; e += 2) {
-        const float a0 = ex2_sel(fmaf(__uint_as_float(s2[e]), sl2, neg_m), e), a1 = ex2_sel(fmaf(__uint_as_float(s2[e + 1]), sl2, neg_m), e + 1);
-        ps2 += a0 + a1;
-        s2[e / 2] = pack_half2(a0, a1);
-      }
-#pragma unroll
-      for (int e = 0; e < 32; e += 2) {
-        const float a0 = ex2_sel(fmaf(__uint_as_float(s3[e]), sl2, neg_m), e), a1 = ex2_sel(fmaf(__uint_as_float(s3[e + 1]), sl2, neg_m), e + 1);
-        ps3 += a0 + a1;
-        s2[16 + e / 2] = pack_half2(a0, a1);
-      }
-      l += (ps0 + ps1) + (ps2 + ps3);
-#endif
-      if (j > 0) {
-        mbar_wait(o_done, (j - 1) & 1);                  // P V of the previous tile retired: P and O may be touched
-        tc_fence_after();
-        if (__any_sync(0xffffffffu, need)) {             // warp-uniform: tcgen05.ld/st are warp-collective
-#pragma unroll 1
-          for (int c = 0; c < 2; ++c) {
-            uint32_t v[32];
-            tmem_ld32(tO + lane_off + c * 32, v);
-            tc_wait_ld();
-#pragma unroll
-            for (int e = 0; e < 32; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) * alpha);
-            tmem_st32(tO + lane_off + c * 32, v);
-          }
-        }
-      }
-      tmem_st32(tP + lane_off, s0);
-      tmem_st32(tP + lane_off + 32, s2);
-      tc_wait_st();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_relaxed(p_full);
-    }
-    // epilogue
-    mbar_wait(o_done, (ntiles - 1) & 1);
-    tc_fence_after();
-    const float inv = 1.f / l;
-    const int row = q0 + r;
-    __half* op = p.out + ((long long)b * p.Nq + row) * p.ldo + head * ATT_D;
-    uint32_t v0[32], v1[32];
-    tmem_ld32(tO + lane_off, v0);
-    tmem_ld32(tO + lane_off + 32, v1);
-    tc_wait_ld();
-    if (row < p.Nq) {
-#pragma unroll
-      for (int g = 0; g < 8; ++g) {
-        float f[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(g < 4 ? v0[g * 8 + e] : v1[(g - 4) * 8 + e]) * inv;
-        uint4* dst = reinterpret_cast<uint4*>(op + g * 8);
-        if (p.accumulate) {
-          const uint4 u = *dst;
-          const __half2* h = reinterpret_cast<const __half2*>(&u);
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float2 t = __half22float2(h[e]);
-            f[2 * e] += t.x; f[2 * e + 1] += t.y;
-          }
-        }
-        uint4 o;
-        o.x = pack_half2(f[0], f[1]); o.y = pack_half2(f[2], f[3]);
-        o.z = pack_half2(f[4], f[5]); o.w = pack_half2(f[6], f[7]);
-        *dst = o;
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
+  // ------------------------------ MMA / softmax warpgroups ------------------------------
+  const int cw = warp >> 2, wl = warp & 3;
+  const uint32_t aQ = smem_u32(sQ) + cw * (64 * ATT_D * 2);
+  const float sl2 = p.scale_log2;
+  float o[32];                                      // O fragments: 64 rows x 64 columns per warpgroup
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};   // rows r0 and r0 + 8 of this thread (l: this thread's partial sum)
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < ntiles; ++j) {
+    const int s = j & 1;
+    const uint32_t aK = smem_u32(sKV + s * 2 * Cfg::KV_BYTES);
+    const uint32_t aV = aK + Cfg::KV_BYTES;
+    mbar_wait(&kv_full[s], (j >> 1) & 1);
+    float sc[BNK / 2];
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < ATT_D / 16; ++k) Wgmma<BNK>::ss(sc, wgmma_desc_sw128(aQ + 32 * k), wgmma_desc_sw128(aK + 32 * k), k > 0 ? 1 : 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(sc);
+
+    const int valid = p.Nk - j * BNK;
+    if (valid < BNK) {
+#pragma unroll
+      for (int i = 0; i < BNK / 2; ++i) {
+        const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+        if (col >= valid) sc[i] = -INFINITY;       // masked keys get probability 0
+      }
+    }
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int i = 0; i < BNK / 2; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], sc[i]);
+    float alpha[2], negm[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+      const float mn = fmaxf(m[h], mx[h] * sl2);
+      alpha[h] = ex2f(m[h] - mn);                   // 0 on the first tile (m = -inf)
+      m[h] = mn;
+      negm[h] = -mn;
+      l[h] *= alpha[h];
+    }
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] *= alpha[(i >> 1) & 1];
+    // probabilities, packed to fp16 A fragments: k-slice kk covers accumulator column groups 2 kk and 2 kk + 1
+    uint32_t pa[BNK / 16][4];
+#pragma unroll
+    for (int kk = 0; kk < BNK / 16; ++kk) {
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const int i = (2 * kk + (r >> 1)) * 4 + 2 * (r & 1);   // r: (row r0, k lo), (row r0+8, k lo), (row r0, k hi), (row r0+8, k hi)
+        const int h = r & 1;
+        const float e0 = ex2f(fmaf(sc[i], sl2, negm[h])), e1 = ex2f(fmaf(sc[i + 1], sl2, negm[h]));
+        l[h] += e0 + e1;
+        pa[kk][r] = pack_half2(e0, e1);
+      }
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BNK / 16; ++kk) Wgmma<64, 1>::rs(o, pa[kk], wgmma_desc_sw128(aV + kk * 16 * 128), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&kv_empty[s]);
+  }
+
+  // epilogue: O / l, rows r0 = 16 wl + lane / 4 and r0 + 8 of the warpgroup's 64
+  float inv[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float t = l[h];
+    t += __shfl_xor_sync(0xffffffffu, t, 1);
+    t += __shfl_xor_sync(0xffffffffu, t, 2);
+    inv[h] = 1.f / t;
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = q0 + cw * 64 + 16 * wl + (lane >> 2) + 8 * h;
+    if (row >= p.Nq) continue;
+    __half* op = p.out + ((long long)b * p.Nq + row) * p.ldo + head * ATT_D + 2 * (lane & 3);
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      float v0 = o[jj * 4 + 2 * h] * inv[h], v1 = o[jj * 4 + 2 * h + 1] * inv[h];
+      __half2* dst = reinterpret_cast<__half2*>(op + 8 * jj);
+      if (p.accumulate) {
+        const float2 t = __half22float2(*dst);
+        v0 += t.x; v1 += t.y;
+      }
+      *dst = __floats2half2_rn(v0, v1);
+    }
   }
 }
 
-int flash_attn_d64(const AttnDesc& d, cudaStream_t stream) {
-  // Short key sequences (text / image cross-attention: 77 / 256 keys; the 18x32 and 9x16 levels: 576 / 144 keys) run on the
-  // 64-key-tile kernel (attention_bn64.cu, three CTAs per SM): measured on B200 (profiles/r02_ab_micro.txt) cross-attention
-  // 179.5 -> 147.1 us (77 keys) and 208.6 -> 186.4 us (256 keys), self-attention at 576 keys 103 -> 87 us; from 2304 keys up the
-  // 128-key tiles of this file win (3.115 vs 3.198 ms at 9216 keys).  VC_ATTN_BN64=1 / 0 forces one kernel.
-  const int bn64 = flash_attn_bn64_mode();
-  if (bn64 == 1 || (bn64 < 0 && d.Nk <= 1024)) return flash_attn_d64_bn64(d, stream);
-  VC_REQUIRE(d.q && d.k && d.v && d.out, "flash_attn: null pointer");
-  VC_REQUIRE(d.Nq > 0 && d.Nk > 0 && d.B > 0 && d.heads > 0, "flash_attn: empty problem");
-  VC_REQUIRE(d.ldq % 8 == 0 && d.ldk % 8 == 0 && d.ldv % 8 == 0 && d.ldo % 8 == 0, "flash_attn: pitches must be multiples of 8");
-  VC_REQUIRE(d.kv_batch_stride % 8 == 0, "flash_attn: kv batch stride must be a multiple of 8");
+// env VC_ATTN_BN64 = 1 / 0 forces the 64- / 128-key tiles for every shape; unset: by key count
+static int bn64_mode() {
+  static int mode = -2;
+  if (mode == -2) { const char* e = getenv("VC_ATTN_BN64"); mode = !e ? -1 : (e[0] == '1' ? 1 : 0); }
+  return mode;
+}
+
+template <int BNK>
+static int launch_attn(const AttnDesc& d, cudaStream_t stream) {
+  using Cfg = AttnCfg<BNK>;
   AttnParams p;
   memset(&p, 0, sizeof(p));
-  uint32_t box[4] = {64, 1, 128, 1};
   {
     uint64_t dims[4] = {64, (uint64_t)d.heads, (uint64_t)d.Nq, (uint64_t)d.B};
     uint64_t str[3] = {128, (uint64_t)d.ldq * 2, (uint64_t)d.ldq * 2 * d.Nq};
+    uint32_t box[4] = {64, 1, ATT_BM, 1};
     int rc = encode_tmap_f16(&p.tmap_q, d.q, 4, dims, str, box);
     if (rc) return rc;
   }
@@ -418,6 +214,7 @@ int flash_attn_d64(const AttnDesc& d, cudaStream_t stream) {
     uint64_t dims[4] = {64, (uint64_t)d.heads, (uint64_t)d.Nk, (uint64_t)(shared ? 1 : d.B)};
     uint64_t strk[3] = {128, (uint64_t)d.ldk * 2, (uint64_t)(shared ? (long long)d.ldk * d.Nk : d.kv_batch_stride) * 2};
     uint64_t strv[3] = {128, (uint64_t)d.ldv * 2, (uint64_t)(shared ? (long long)d.ldv * d.Nk : d.kv_batch_stride) * 2};
+    uint32_t box[4] = {64, 1, (uint32_t)BNK, 1};
     int rc = encode_tmap_f16(&p.tmap_k, d.k, 4, dims, strk, box);
     if (rc) return rc;
     rc = encode_tmap_f16(&p.tmap_v, d.v, 4, dims, strv, box);
@@ -428,13 +225,23 @@ int flash_attn_d64(const AttnDesc& d, cudaStream_t stream) {
   p.accumulate = d.accumulate;
   static DeviceOnce configured;
   if (device_once_needed(configured)) {
-    VC_CHECK_CUDA(cudaFuncSetAttribute(flash_attn_d64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
+    VC_CHECK_CUDA(cudaFuncSetAttribute(flash_attn_d64_kernel<BNK>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM));
     device_once_mark(configured);
   }
   dim3 grid((d.Nq + ATT_BM - 1) / ATT_BM, d.heads, d.B);
-  flash_attn_d64_kernel<<<grid, 192, ATT_SMEM, stream>>>(p);
+  flash_attn_d64_kernel<BNK><<<grid, ATT_THREADS, Cfg::SMEM, stream>>>(p);
   VC_CHECK_CUDA(cudaGetLastError());
   return VC_OK;
+}
+
+int flash_attn_d64(const AttnDesc& d, cudaStream_t stream) {
+  VC_REQUIRE(d.q && d.k && d.v && d.out, "flash_attn: null pointer");
+  VC_REQUIRE(d.Nq > 0 && d.Nk > 0 && d.B > 0 && d.heads > 0, "flash_attn: empty problem");
+  VC_REQUIRE(d.ldq % 8 == 0 && d.ldk % 8 == 0 && d.ldv % 8 == 0 && d.ldo % 8 == 0, "flash_attn: pitches must be multiples of 8");
+  VC_REQUIRE(d.kv_batch_stride % 8 == 0, "flash_attn: kv batch stride must be a multiple of 8");
+  const int mode = bn64_mode();
+  if (mode == 1 || (mode < 0 && d.Nk <= 1024)) return launch_attn<64>(d, stream);
+  return launch_attn<128>(d, stream);
 }
 
 }  // namespace vc

@@ -1,12 +1,14 @@
 #!/bin/bash
-# Build libvc_b200.so in-tree for sm_100a (cross-compiles without a GPU).
+# Build libvc_b200.so in-tree for sm_90a (H100; cross-compiles without a GPU).
 set -euo pipefail
 cd "$(dirname "$0")"
-NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
-FLAGS="-gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -Xcompiler -Wall --expt-relaxed-constexpr ${VC_NVCC_EXTRA:-}"
+NVCC=${NVCC:-nvcc}
+if ! command -v "$NVCC" >/dev/null 2>&1 && [ -x /usr/local/cuda/bin/nvcc ]; then NVCC=/usr/local/cuda/bin/nvcc; fi
+ARCH="-gencode arch=compute_90a,code=sm_90a"
+FLAGS="$ARCH -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -Xcompiler -Wall --expt-relaxed-constexpr ${VC_NVCC_EXTRA:-}"
 OUT=${VC_OUT:-../libvc_b200.so}          # VC_OUT / VC_BUILD_DIR / VC_NVCC_EXTRA: side-by-side A/B builds (load with VC_B200_LIB)
 BUILD=${VC_BUILD_DIR:-build}
-SRCS="host.cu capi.cu gemm_tap.cu gemm_tap2.cu attention.cu attention_bn64.cu temporal_attn.cu norm.cu misc.cu peer.cu"
+SRCS="host.cu capi.cu gemm_tap.cu attention.cu temporal_attn.cu norm.cu misc.cu peer.cu"
 mkdir -p $BUILD
 pids=()
 for f in $SRCS; do
@@ -14,5 +16,5 @@ for f in $SRCS; do
   pids+=($!)
 done
 for p in "${pids[@]}"; do wait $p; done
-$NVCC -gencode arch=compute_100a,code=sm_100a -shared -o $OUT $BUILD/*.o -lcudart
+$NVCC $ARCH -shared -o $OUT $BUILD/*.o -lcudart
 echo "built $(realpath $OUT)"

@@ -1,5 +1,5 @@
-// Shared device/host helpers for the sm_100a kernels: mbarrier, TMA, tcgen05 (UMMA/TMEM) PTX wrappers,
-// UMMA descriptors, tensor-map encoding through the driver entry point (no libcuda link dependency).
+// Shared device/host helpers for the sm_90a kernels: mbarrier, TMA and wgmma PTX wrappers,
+// wgmma descriptors, tensor-map encoding through the driver entry point (no libcuda link dependency).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -85,13 +85,6 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-// Arrival WITHOUT release semantics: for hand-offs whose payload lives in TMEM (ordered by tcgen05.fence::before/after
-// around the barrier).  The default .release form compiles to MEMBAR.ALL.CTA, which makes the arriving warp wait until
-// all of its earlier *global stores* have drained -- a ~1 us bubble per tile in a GEMM epilogue (seen in ncu: MEMBAR /
-// ERRBAR among the top stall PCs).
-__device__ __forceinline__ void mbar_arrive_relaxed(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.relaxed.cta.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)));
-}
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -107,25 +100,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) {
   }
 }
-// Wait for warps with slack (TMA producer, MMA issuer of the attention kernel): try_wait with a suspend-time hint, which
-// compiles to SYNCS.TRYWAIT + NANOSLEEP.SYNCS (the warp sleeps until the barrier event or the time limit).
-// A bare try_wait loop re-issues every ~20 cycles (ncu: 44 M + 38 M TRYWAIT executions in one
-// attention launch, 11 % of all issued instructions) and those warps share schedulers 0/1 with two of the four softmax
-// warps, whose issue slots they take.
-__device__ __forceinline__ void mbar_wait_parked(uint64_t* bar, uint32_t parity) {
-  for (;;) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred P1;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%1], %2, %3;\n\t"
-        "selp.b32 %0, 1, 0, P1;\n\t}\n"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity), "r"(2000u)
-        : "memory");
-    if (ok) return;
-  }
-}
-
 // ---- TMA (cp.async.bulk.tensor) ----
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
@@ -161,88 +135,33 @@ __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bu
 // make generic-proxy shared-memory writes visible to the async proxy (TMA) before it reads them
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ---- tcgen05 / TMEM ----
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
+// ---- wgmma (warpgroup MMA, sm_90a) ----
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keep the accumulator registers live across the asynchronous MMAs (no reordering of their reads / writes around the fence)
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+// named barrier over `count` threads (one id per warpgroup; id 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
-// tcgen05.commit: arrives (count 1) on the mbarrier once all previously issued MMAs of this thread retire.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// D[tmem] (+)= A[smem] * B[smem]; kind::f16 (fp16/bf16 in, fp32 accumulate)
-__device__ __forceinline__ void umma_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// Instruction descriptor for kind::f16: fp16 A/B, fp32 D.  a_mn/b_mn: 1 = MN-major operand.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N, int a_mn = 0, int b_mn = 0) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// Shared-memory matrix descriptor, 128B swizzle, rows of 128 bytes (64 fp16) stored densely:
+// Shared-memory matrix descriptor, 128B swizzle, rows of 128 bytes (64 fp16) stored densely, as TMA writes them with
+// CU_TENSOR_MAP_SWIZZLE_128B:
 //   K-major operand  (tile [rows][64 k]):  SBO = 1024 B between 8-row groups, LBO unused (=1).
-//   MN-major operand (tile [k rows][64 mn]): same geometry: each k-row holds 64 contiguous MN elements.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes = 16, uint32_t sbo_bytes = 1024) {
+//   MN-major operand (tile [k rows][64 mn]): SBO = 1024 B between 8-row (k) groups, LBO = distance between 64-wide mn blocks.
+// Advancing along K by 16 elements inside a 128-byte row adds 32 bytes to the start address (the swizzle is applied by
+// the hardware on absolute address bits, so tiles must be 1024-byte aligned).
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes = 16, uint32_t sbo_bytes = 1024) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;   // descriptor version for sm_100
-  d |= (uint64_t)2 << 61;   // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;   // SWIZZLE_128B
   return d;
-}
-
-// TMEM -> registers: this warp's 32 lanes (lane quadrant = warp_id % 4), 32 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-// registers -> TMEM, 32 consecutive 32-bit columns of this thread's lane.
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
 }
 
 __device__ __forceinline__ uint32_t pack_half2(float a, float b) {

@@ -1,5 +1,5 @@
-// Shared pieces of the tap-GEMM kernels (gemm_tap.cu: one CTA per tile, gemm_tap2.cu: CTA pair per 256-row tile):
-// parameter block, tile enumeration and the TMEM -> registers -> global epilogue.
+// Shared pieces of the tap-GEMM kernel (gemm_tap.cu): parameter block, tile enumeration and the per-chunk epilogue
+// (bias / folded LayerNorm / residual / statistics / store) that runs on one output row x 32 columns per thread.
 #pragma once
 #include "common.cuh"
 
@@ -8,15 +8,17 @@ namespace vc {
 static constexpr int BM = 128;
 static constexpr int BK = 64;
 static constexpr int MAX_TAPS = 9;
-#ifndef VC_EPI_WARPS
-#define VC_EPI_WARPS 12
-#endif
-static constexpr int EPI_WARPS = VC_EPI_WARPS;   // multiple of 4 (EPI_WARPS / 4 warps per TMEM lane quadrant).  12 warps -> 14 per CTA -> 128 registers
-                                                 // per thread without spills; 16 warps cap at 96 and spilled the residual prefetch (measured slower)
-static constexpr int EPI_PER_QUAD = EPI_WARPS / 4;
-static constexpr int GEMM_THREADS = 64 + EPI_WARPS * 32;
+// one producer warpgroup (TMA) + two MMA warpgroups, each owning 64 of the tile's 128 rows
+static constexpr int MMA_WGS = 2;
+static constexpr int GEMM_THREADS = 128 * (1 + MMA_WGS);
+static constexpr int EPI_WARPS = 4 * MMA_WGS;
 static constexpr int EPI_STAGE_BYTES = 32 * 32 * 2;              // one warp's staging tile for TMA stores: 32 rows x 32 fp16
-static constexpr int EPI_SMEM_BYTES = EPI_WARPS * EPI_STAGE_BYTES;
+// accumulator transpose: an MMA warpgroup writes 64 rows x 64 columns of fp32 at a time, then each warp reads back 32 rows x
+// 32 columns with one row per thread.  Row pitch 72 floats: the fragment writes (8 rows x 4 column pairs per warp) hit 32
+// distinct banks per half warp.
+static constexpr int EPI_XPOSE_PITCH = 72;
+static constexpr int EPI_XPOSE_BYTES = 64 * EPI_XPOSE_PITCH * 4;
+static constexpr int EPI_SMEM_BYTES = EPI_WARPS * EPI_STAGE_BYTES + MMA_WGS * EPI_XPOSE_BYTES;
 
 // Division by a runtime constant as multiply-high + shift (valid for dividends < 2^31): the persistent kernels turn a
 // linear tile index into (n-tile, x, y, z) once per tile in EVERY thread, and a generic 32-bit division is ~20 SASS
@@ -37,16 +39,6 @@ static inline FastDiv make_fastdiv(int d) {
 }
 #ifdef __CUDACC__
 __device__ __forceinline__ int fast_div(const FastDiv& f, int n) { return f.d == 1 ? n : (int)(__umulhi((uint32_t)n, f.mul) >> f.shr); }
-#endif
-
-// the profiling branches are compiled out of the shipped kernels (they sat inside the producer / MMA / epilogue loops)
-#ifndef VC_GEMM_DEBUG_BUILD
-#define VC_GEMM_DEBUG_BUILD 0
-#endif
-#if VC_GEMM_DEBUG_BUILD
-#define VC_GEMM_DBG(p, bit) ((p).debug & (bit))
-#else
-#define VC_GEMM_DBG(p, bit) 0
 #endif
 
 // Multi-GPU layout switch fused into the epilogue (frame-sharded U-Net, parallel.py): instead of writing its output locally and
@@ -83,7 +75,7 @@ struct GemmParams {
   int tap_dx[MAX_TAPS];
   int tap_dy[MAX_TAPS];
   int n_tiles;
-  int total_tiles;       // 1-CTA kernel: m_tiles * n_tiles; pair kernel: ceil(m_tiles / 2) * n_tiles
+  int total_tiles;       // m_tiles * n_tiles
   __half* out;
   float* out_f32;
   int ldo;
@@ -102,15 +94,13 @@ struct GemmParams {
   int out_tma;           // fp16 output written by TMA stores from per-warp staging tiles (full-line, LSU-free)
   int vec_ok;            // rows are 32-byte aligned: the 256-bit epilogue path may be used
   GemmPeer peer;         // output scattered to the ranks of the frame group (mode != 0: `out` itself is not written)
-  int debug;             // profiling aid, only honoured by builds with -DVC_GEMM_DEBUG_BUILD=1 (env VC_GEMM_DEBUG): 1 = skip the MMAs
-                         // (feed rate only), 2 = skip TMA (MMA rate only), 4 = skip the epilogue body; results are garbage then
 };
 
 struct TileCoord {
   int x0, y0, z;
 };
 
-// m-tile index -> tile origin; indices past the last m-tile give z >= Z (TMA zero-fills, the epilogue masks the rows)
+// m-tile index -> tile origin
 #ifdef __CUDACC__
 __device__ __forceinline__ TileCoord tile_coord_m(const GemmParams& p, int m) {
   TileCoord t;
@@ -125,19 +115,6 @@ __device__ __forceinline__ TileCoord tile_coord_m(const GemmParams& p, int m) {
 #endif
 
 #ifdef __CUDACC__
-// 256-bit global accesses (sm_100: LDG/STG.E.ENL2.256): one instruction moves a full 32-byte sector per thread
-__device__ __forceinline__ void st_global_256(void* ptr, const uint32_t (&v)[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(ptr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]),
-               "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
-}
-__device__ __forceinline__ void ld_global_256(const void* ptr, uint32_t (&v)[8]) {
-  asm volatile("ld.global.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "l"(ptr)
-               : "memory");
-}
-
 // exact-erf GELU (attention.py:415-422 uses F.gelu), erf by Abramowitz-Stegun 7.1.26 (|err| < 1.5e-7): 2 MUFU + ~12 FMA/ALU
 __device__ __forceinline__ float gelu_epilogue(float x) {
   const float z = x * 0.70710678118654752440f;
@@ -155,79 +132,40 @@ __device__ __forceinline__ float gelu_epilogue(float x) {
   return fmaf(hx, copysignf(erf_abs, z), hx);
 }
 
-// the same arithmetic on two gate values at once in packed fp32x2 (FMUL2 / FFMA2, sm_100): the GEGLU epilogue was issue-bound
-// (ncu round 1: 34 instructions per output, tensor pipe 41 %); per pair: 12 packed FP ops + 4 MUFU + 4 LOP3 instead of 26 + 4 + 2
-__device__ __forceinline__ float2 gelu_epilogue2(float2 x) {
-  const float2 z = __fmul2_rn(x, make_float2(0.70710678118654752440f, 0.70710678118654752440f));
-  const float2 az = make_float2(fabsf(z.x), fabsf(z.y));
-  const float2 den = __ffma2_rn(make_float2(0.3275911f, 0.3275911f), az, make_float2(1.0f, 1.0f));
-  float2 t;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t.x) : "f"(den.x));
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t.y) : "f"(den.y));
-  float2 poly = __ffma2_rn(make_float2(1.061405429f, 1.061405429f), t, make_float2(-1.453152027f, -1.453152027f));
-  poly = __ffma2_rn(poly, t, make_float2(1.421413741f, 1.421413741f));
-  poly = __ffma2_rn(poly, t, make_float2(-0.284496736f, -0.284496736f));
-  poly = __ffma2_rn(poly, t, make_float2(0.254829592f, 0.254829592f));
-  const float2 earg = __fmul2_rn(__fmul2_rn(az, az), make_float2(-1.4426950408889634f, -1.4426950408889634f));
-  float2 e;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e.x) : "f"(earg.x));
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e.y) : "f"(earg.y));
-  const float2 npt = __fmul2_rn(poly, make_float2(-t.x, -t.y));
-  const float2 erf_abs = __ffma2_rn(npt, e, make_float2(1.0f, 1.0f));
-  const float2 hx = __fmul2_rn(x, make_float2(0.5f, 0.5f));
-  return __ffma2_rn(hx, make_float2(copysignf(erf_abs.x, z.x), copysignf(erf_abs.y, z.y)), hx);
-}
-
 // ---------------------------------------------------------------------------------------------------------------
-// Epilogue: TMEM -> registers -> (+bias / GEGLU / +residual) -> 256-bit global stores (whole 32-byte sectors), executed
-// by the EPI_WARPS epilogue warps (warp index 2..) of both GEMM kernels.  EPI_PER_QUAD warps share each TMEM lane
-// quadrant and split the accumulator's 32-column chunks; each thread owns one row.
-//   * chunk ownership rotates with the CTA-local tile counter `lt`, so tiles whose chunk count is not a multiple of
-//     EPI_PER_QUAD load the warps evenly over consecutive tiles;
-//   * the residual is software-pipelined one chunk ahead ACROSS tiles: while a chunk is converted and stored, the
-//     residual of the warp's next chunk -- of this tile or of the CTA's next tile -- is already in flight, so its HBM
-//     latency overlaps the main loop instead of sitting on the epilogue's critical path (measured: short-K linears with a
-//     residual spent a quarter of all epilogue stall samples on that load).
+// Epilogue chunk: one thread owns one output row and 32 consecutive columns (the accumulator was transposed through shared
+// memory by gemm_tap_kernel), a warp owns 32 consecutive rows of the tile: quad = 32-row block of the 128-row tile.
 // ---------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ int epi_first_chunk(int sub, int lt, int nch) {
-  // chunk g = lt * nch + c of the CTA's chunk stream belongs to warp slot g mod EPI_PER_QUAD
-  if ((EPI_PER_QUAD & (EPI_PER_QUAD - 1)) == 0) return (sub - lt * nch) & (EPI_PER_QUAD - 1);
-  const int m = (lt * nch) % EPI_PER_QUAD;
-  return (sub + EPI_PER_QUAD - m) % EPI_PER_QUAD;
-}
-
 struct EpiTile {
   long long orow;        // output row index of this thread
   const float* bias;     // bias row for this tile's z (or nullptr)
   int n_tile;
   int m_tile;            // linear m-tile index (x fastest, then y, then z)
-  int c_first;           // this warp's first chunk in the tile
+  int quad;              // 32-row block of the tile owned by this warp
   int wx, wy, wz;        // (x, y, z) of the warp's first row: TMA store coordinates
   bool row_ok;
 };
 
-// tile index -> this thread's view of it.  m-tile = (tile / n_tiles) * m_mul + m_add  (CTA pairs: m_mul 2, m_add rank)
-__device__ __forceinline__ EpiTile epi_tile(const GemmParams& p, int tile, int lt, int nch, int m_mul, int m_add, int warp, int lane) {
+__device__ __forceinline__ EpiTile epi_tile(const GemmParams& p, int tile, int quad, int lane) {
   EpiTile t;
   const int mq = fast_div(p.div_n_tiles, tile);
   t.n_tile = tile - mq * p.n_tiles;
-  t.m_tile = mq * m_mul + m_add;
+  t.m_tile = mq;
+  t.quad = quad;
   const TileCoord tc = tile_coord_m(p, t.m_tile);
-  const int R = (warp & 3) * 32 + lane;          // accumulator row owned by this thread (TMEM lane)
-  const int R0 = (warp & 3) * 32;
+  const int R = quad * 32 + lane;                // tile row owned by this thread
+  const int R0 = quad * 32;
   t.wx = tc.x0 + (R0 & (p.bx - 1)); t.wy = tc.y0 + (R0 >> p.bx_shift); t.wz = tc.z;
   const int x = tc.x0 + (R & (p.bx - 1)), y = tc.y0 + (R >> p.bx_shift);
   t.row_ok = x < p.X && y < p.Y && tc.z < p.Z;
   t.orow = ((long long)tc.z * p.Y + y) * p.X + x;
   t.bias = p.bias ? p.bias + (long long)(p.bias_z_div > 0 ? min(tc.z, p.Z - 1) / p.bias_z_div : 0) * p.N : nullptr;
-  t.c_first = epi_first_chunk((warp - 2) >> 2, lt, nch);
   return t;
 }
 
 // peer mode: the warp's staged 32 x 32 tile goes to the rank(s) owning its rows in the other layout (executed by one lane)
 __device__ __forceinline__ void peer_scatter32(const GemmParams& p, const EpiTile& t, int col0, const uint8_t* stage) {
   const GemmPeer& g = p.peer;
-  if (t.wz >= p.Z) return;                     // the padding m-tile of an odd tile count (CTA pairs): its coordinates wrap to (x0 = 0, z = Z)
   int lin = t.wy * p.X + t.wx;                 // first row of the warp's patch inside its z-slab (patches are row-contiguous: host check)
   int slab = t.wz;
   if (g.wrap) { slab = fast_div(g.div_rps, lin); lin -= slab * g.rps; }
@@ -259,8 +197,8 @@ __device__ __forceinline__ void epi_store32(const GemmParams& p, const EpiTile& 
                                             uint8_t* stage, int lane) {
   if (p.out_tma) {
     // Stage the warp's 32 x 32 fp16 tile in shared memory (64B-swizzled rows: conflict-free 16-byte stores) and let the TMA
-    // unit write it: rows outside (X, Y, Z) are clipped by the tensor map, the LSU sees no global store at all.  Row-per-
-    // thread 32-byte global stores touch 32 different 128-byte lines per instruction and capped the epilogue at ~3 TB/s.
+    // unit write it: rows outside (X, Y, Z) are clipped by the tensor map.  Row-per-thread global stores would touch 32
+    // different 128-byte lines per instruction.
     if (lane == 0) tma_store_wait_read();          // the previous store has finished reading this warp's staging tile
     __syncwarp();
     const uint32_t sbase = smem_u32(stage) + lane * 64;
@@ -283,23 +221,15 @@ __device__ __forceinline__ void epi_store32(const GemmParams& p, const EpiTile& 
   if (!t.row_ok || col0 >= n_out) return;
   if (col0 + 32 <= n_out && p.vec_ok) {
     if (p.out_f32) {
-      float* op = p.out_f32 + t.orow * p.ldo + col0;
+      float4* op = reinterpret_cast<float4*>(p.out_f32 + t.orow * p.ldo + col0);
 #pragma unroll
-      for (int h = 0; h < 4; ++h) {
-        uint32_t u[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) u[e] = __float_as_uint(f[h * 8 + e]);
-        st_global_256(op + h * 8, u);
-      }
+      for (int h = 0; h < 8; ++h) op[h] = make_float4(f[h * 4], f[h * 4 + 1], f[h * 4 + 2], f[h * 4 + 3]);
     } else {
-      __half* op = p.out + t.orow * p.ldo + col0;
+      uint4* op = reinterpret_cast<uint4*>(p.out + t.orow * p.ldo + col0);
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        uint32_t u[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) u[e] = pack_half2(f[h * 16 + 2 * e], f[h * 16 + 2 * e + 1]);
-        st_global_256(op + h * 16, u);
-      }
+      for (int h = 0; h < 4; ++h)
+        op[h] = make_uint4(pack_half2(f[h * 8 + 0], f[h * 8 + 1]), pack_half2(f[h * 8 + 2], f[h * 8 + 3]), pack_half2(f[h * 8 + 4], f[h * 8 + 5]),
+                           pack_half2(f[h * 8 + 6], f[h * 8 + 7]));
     }
   } else {
     // ragged N tail / unaligned pitch (e.g. the 320->4 output conv): predicated scalar path
@@ -327,23 +257,23 @@ __device__ __forceinline__ void epi_store32(const GemmParams& p, const EpiTile& 
 // B1 = pairs in the first piece, HP = pairs per sub-group.
 template <int B1, int HP>
 __device__ __forceinline__ void gn_piece_sums(const float (&f)[32], bool row_ok, float (&v)[8]) {
-  float2 s[4], q[4];
+  float s[4], q[4];
 #pragma unroll
-  for (int i = 0; i < 4; ++i) s[i] = q[i] = make_float2(0.f, 0.f);
+  for (int i = 0; i < 4; ++i) s[i] = q[i] = 0.f;
 #pragma unroll
   for (int e = 0; e < 16; ++e) {
     const int piece = e < B1 ? 0 : e < B1 + HP ? 1 : e < B1 + 2 * HP ? 2 : 3;
     const float2 r = __half22float2(__floats2half2_rn(f[2 * e], f[2 * e + 1]));
-    s[piece] = __fadd2_rn(s[piece], r);
-    q[piece] = __ffma2_rn(r, r, q[piece]);
+    s[piece] += r.x + r.y;
+    q[piece] = fmaf(r.x, r.x, fmaf(r.y, r.y, q[piece]));
   }
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
-    v[i] = row_ok ? s[i].x + s[i].y : 0.f;
-    v[4 + i] = row_ok ? q[i].x + q[i].y : 0.f;
+    v[i] = row_ok ? s[i] : 0.f;
+    v[4 + i] = row_ok ? q[i] : 0.f;
   }
 }
-__device__ __forceinline__ void gn_part_accumulate(const GemmParams& p, const EpiTile& t, int nb, const float (&f)[32], int warp, int lane) {
+__device__ __forceinline__ void gn_part_accumulate(const GemmParams& p, const EpiTile& t, int nb, const float (&f)[32], int lane) {
   float v[8];
   const int sub = 2 * p.gn_hp;
   const int o = nb % sub;                               // even: nb is a multiple of 32, sub is even
@@ -385,207 +315,69 @@ __device__ __forceinline__ void gn_part_accumulate(const GemmParams& p, const Ep
   // lane bits (4, 3, 2) select which of the 8 numbers this lane ended up with: idx = 4*b4 + 2*b3 + b2  (0..3 sums, 4..7 sums of squares)
   if ((lane & 3) == 0) {
     const int idx = ((lane >> 4) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 2) & 1);
-    const long long rb = (long long)t.m_tile * 4 + (warp & 3);
+    const long long rb = (long long)t.m_tile * 4 + t.quad;
     float* dst = reinterpret_cast<float*>(p.gn_part + (rb * p.gn_nchunks + (nb >> 5)) * 4);
     dst[(idx & 3) * 2 + (idx >> 2)] = v[0];
   }
 }
 
-// is chunk c of tile t on the vectorised residual path?  (same predicate at prefetch and at use)
-template <int BN>
-__device__ __forceinline__ bool epi_res_vec(const GemmParams& p, const EpiTile& t, int c) {
-  return p.res != nullptr && p.vec_ok && t.row_ok && c < BN / 32 && t.n_tile * BN + c * 32 + 32 <= p.N;
-}
-template <int BN>
-__device__ __forceinline__ void epi_res_prefetch(const GemmParams& p, const EpiTile& t, int c, uint32_t (&rres)[16]) {
-  if (epi_res_vec<BN>(p, t, c)) {
-    const __half* rp = p.res + t.orow * p.ldr + t.n_tile * BN + c * 32;   // plain loads: res may alias out (in-place residual)
-    ld_global_256(rp, *reinterpret_cast<uint32_t(*)[8]>(&rres[0]));
-    ld_global_256(rp + 16, *reinterpret_cast<uint32_t(*)[8]>(&rres[8]));
-  }
-}
-
-// hand a drained accumulator back to the MMA warp (CTA pairs: to the leader CTA's barrier).  Relaxed: the payload is TMEM,
-// ordered by the tcgen05 fences; a release here would be a MEMBAR that waits for the warp's outstanding global stores.
-template <bool PAIR>
-__device__ __forceinline__ void epi_release_acc(uint64_t* bar) {
-  if (PAIR) {
-    uint32_t remote;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(0u));
-    asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote));
-  } else {
-    mbar_arrive_relaxed(bar);
-  }
-}
-
-// The epilogue warps' whole persistent loop over this CTA's tiles tile0, tile0 + stride, ... < p.total_tiles.
-template <int BN, int NACC, bool PAIR>
-__device__ __forceinline__ void gemm_epilogue_loop(const GemmParams& p, int tile0, int stride, int m_mul, int m_add, uint32_t tmem_base,
-                                                   uint64_t* tmem_full_bar, uint64_t* tmem_empty_bar, uint8_t* epi_smem, int warp,
-                                                   int lane) {
-  uint8_t* stage = epi_smem + (warp - 2) * EPI_STAGE_BYTES;
-  const uint32_t tquad = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
-  int acc = 0, lt = 0;
-  uint32_t aph = 0;
-  if (!p.geglu) {
-    constexpr int NCH = BN / 32;
-    constexpr int MAXC = (NCH + EPI_PER_QUAD - 1) / EPI_PER_QUAD;
-    if (tile0 >= p.total_tiles) return;
-    EpiTile cur = epi_tile(p, tile0, 0, NCH, m_mul, m_add, warp, lane);
-    uint32_t rres[16];
-    epi_res_prefetch<BN>(p, cur, cur.c_first, rres);
-    for (int tile = tile0; tile < p.total_tiles; tile += stride, ++lt) {
-      const bool has_next = tile + stride < p.total_tiles;
-      EpiTile nxt = cur;
-      if (has_next) nxt = epi_tile(p, tile + stride, lt + 1, NCH, m_mul, m_add, warp, lane);
-      const int n0 = cur.n_tile * BN;
-      // chunks of this warp in this tile: c_first + j * EPI_PER_QUAD while inside the tile and inside N
-      int nmy = 0;
+// One 32-column chunk of this thread's row: folded LayerNorm, bias, residual, output statistics, store.
+// nb: first column in the accumulator's N space (bias / LayerNorm column sums / residual / statistics), col0: first output column.
+// plain: the values are final already (GEGLU, computed on the fragments), only statistics-free storing remains.
+__device__ __forceinline__ void epi_chunk(const GemmParams& p, const EpiTile& t, int nb, int col0, int n_out, bool plain, float (&f)[32],
+                                          uint8_t* stage, int lane) {
+  bool res_vec = false;
+  if (!plain) {
+    if (p.ln_stats) {                              // folded LayerNorm (host guarantees N % 32 == 0)
+      const float2 ln = t.row_ok ? __ldg(reinterpret_cast<const float2*>(p.ln_stats) + t.orow) : make_float2(0.f, 1.f);
 #pragma unroll
-      for (int j = 0; j < MAXC; ++j) {
-        const int c = cur.c_first + j * EPI_PER_QUAD;
-        if (c < NCH && n0 + c * 32 < p.N) nmy = j + 1;
+      for (int e = 0; e < 32; e += 4) {
+        const float4 cs = __ldg(reinterpret_cast<const float4*>(p.ln_colsum + nb + e));
+        f[e] = (f[e] - ln.x * cs.x) * ln.y; f[e + 1] = (f[e + 1] - ln.x * cs.y) * ln.y;
+        f[e + 2] = (f[e + 2] - ln.x * cs.z) * ln.y; f[e + 3] = (f[e + 3] - ln.x * cs.w) * ln.y;
       }
-      if (nmy == 0 && has_next) epi_res_prefetch<BN>(p, nxt, nxt.c_first, rres);
-      float2 ln = make_float2(0.f, 1.f);
-      if (p.ln_stats && cur.row_ok) ln = __ldg(reinterpret_cast<const float2*>(p.ln_stats) + cur.orow);
-
-      mbar_wait(&tmem_full_bar[acc], aph);          // accumulator complete
-      tc_fence_after();
-      if (!VC_GEMM_DBG(p, 4)) {
+    }
+    if (t.bias) {
+      if (nb + 32 <= p.N) {
 #pragma unroll
-        for (int j = 0; j < MAXC; ++j) {
-          if (j >= nmy) break;                       // warp-uniform
-          const int c = cur.c_first + j * EPI_PER_QUAD;
-          const int nb = n0 + c * 32;
-          float f[32];
-          {
-            uint32_t v[32];
-            __syncwarp();
-            tmem_ld32(tquad + acc * BN + c * 32, v);
-            tc_wait_ld();
+        for (int e = 0; e < 32; e += 4) {
+          const float4 b4 = __ldg(reinterpret_cast<const float4*>(t.bias + nb + e));
+          f[e] += b4.x; f[e + 1] += b4.y; f[e + 2] += b4.z; f[e + 3] += b4.w;
+        }
+      } else {
 #pragma unroll
-            for (int e = 0; e < 32; ++e) f[e] = __uint_as_float(v[e]);
-          }
-          if (p.ln_stats) {                          // folded LayerNorm (host guarantees N % 32 == 0); packed fp32x2
-            const float2 nm2 = make_float2(-ln.x, -ln.x), rs2 = make_float2(ln.y, ln.y);
+        for (int e = 0; e < 32; ++e)
+          if (nb + e < p.N) f[e] += __ldg(t.bias + nb + e);
+      }
+    }
+    res_vec = p.res != nullptr && p.vec_ok && t.row_ok && nb + 32 <= p.N;
+    if (res_vec) {
+      const uint4* rp = reinterpret_cast<const uint4*>(p.res + t.orow * p.ldr + nb);   // plain loads: res may alias out (in-place residual)
 #pragma unroll
-            for (int e = 0; e < 32; e += 4) {
-              const float4 cs = __ldg(reinterpret_cast<const float4*>(p.ln_colsum + nb + e));
-              const float2 r01 = __fmul2_rn(__ffma2_rn(nm2, make_float2(cs.x, cs.y), make_float2(f[e], f[e + 1])), rs2);
-              const float2 r23 = __fmul2_rn(__ffma2_rn(nm2, make_float2(cs.z, cs.w), make_float2(f[e + 2], f[e + 3])), rs2);
-              f[e] = r01.x; f[e + 1] = r01.y; f[e + 2] = r23.x; f[e + 3] = r23.y;
-            }
-          }
-          if (cur.bias) {
-            if (nb + 32 <= p.N) {
+      for (int h = 0; h < 4; ++h) {
+        const uint4 u = rp[h];
+        const __half2* r2 = reinterpret_cast<const __half2*>(&u);
 #pragma unroll
-              for (int e = 0; e < 32; e += 4) {
-                const float4 b4 = __ldg(reinterpret_cast<const float4*>(cur.bias + nb + e));
-                const float2 r01 = __fadd2_rn(make_float2(f[e], f[e + 1]), make_float2(b4.x, b4.y));
-                const float2 r23 = __fadd2_rn(make_float2(f[e + 2], f[e + 3]), make_float2(b4.z, b4.w));
-                f[e] = r01.x; f[e + 1] = r01.y; f[e + 2] = r23.x; f[e + 3] = r23.y;
-              }
-            } else {
-#pragma unroll
-              for (int e = 0; e < 32; ++e)
-                if (nb + e < p.N) f[e] += __ldg(cur.bias + nb + e);
-            }
-          }
-          const bool vec = epi_res_vec<BN>(p, cur, c);
-          if (vec) {
-#pragma unroll
-            for (int e = 0; e < 16; ++e) {
-              const float2 r = __fadd2_rn(make_float2(f[2 * e], f[2 * e + 1]), __half22float2(*reinterpret_cast<const __half2*>(&rres[e])));
-              f[2 * e] = r.x; f[2 * e + 1] = r.y;
-            }
-          }
-          // rres is free again: request the residual of this warp's next chunk before storing this one
-          if (j + 1 < nmy) epi_res_prefetch<BN>(p, cur, c + EPI_PER_QUAD, rres);
-          else if (has_next) epi_res_prefetch<BN>(p, nxt, nxt.c_first, rres);
-          if (p.ln_part) {                           // LayerNorm statistics of the OUTPUT row, as stored (fp16-rounded)
-            float2 s2 = make_float2(0.f, 0.f), q2 = s2;
-#pragma unroll
-            for (int e = 0; e < 32; e += 2) {
-              const float2 r = __half22float2(__floats2half2_rn(f[e], f[e + 1]));
-              s2 = __fadd2_rn(s2, r);
-              q2 = __ffma2_rn(r, r, q2);
-            }
-            if (cur.row_ok) p.ln_part[(long long)(nb >> 5) * p.ln_rows + cur.orow] = make_float2(s2.x + s2.y, q2.x + q2.y);
-          }
-          if (p.gn_part) gn_part_accumulate(p, cur, nb, f, warp, lane);
-          epi_store32(p, cur, nb, p.N, f, p.res != nullptr && !vec, stage, lane);
+        for (int e = 0; e < 4; ++e) {
+          const float2 r = __half22float2(r2[e]);
+          f[h * 8 + 2 * e] += r.x; f[h * 8 + 2 * e + 1] += r.y;
         }
       }
-      // all TMEM reads of this accumulator are complete (tcgen05.wait::ld above): hand it back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) epi_release_acc<PAIR>(&tmem_empty_bar[acc]);
-      if (++acc == NACC) { acc = 0; aph ^= 1; }
-      cur = nxt;
     }
-  } else {
-    // GEGLU: tile columns [0,BN/2) are values, [BN/2,BN) the matching gates (weights were interleaved per tile);
-    // out[:, n_tile*BN/2 + c] = (value + bias_v) * gelu(gate + bias_g).  No residual (checked on the host).
-    constexpr int HALF = BN / 2;
-    constexpr int NCH = HALF / 32 > 0 ? HALF / 32 : 1;
-    constexpr int MAXC = (NCH + EPI_PER_QUAD - 1) / EPI_PER_QUAD;
-    for (int tile = tile0; tile < p.total_tiles; tile += stride, ++lt) {
-      const EpiTile cur = epi_tile(p, tile, lt, NCH, m_mul, m_add, warp, lane);
-      const int n0 = cur.n_tile * BN;
-      float2 ln = make_float2(0.f, 1.f);
-      if (p.ln_stats && cur.row_ok) ln = __ldg(reinterpret_cast<const float2*>(p.ln_stats) + cur.orow);
-      const float nm = -ln.x;
-      mbar_wait(&tmem_full_bar[acc], aph);
-      tc_fence_after();
-      if (!VC_GEMM_DBG(p, 4)) {
+    if (p.ln_part) {                               // LayerNorm statistics of the OUTPUT row, as stored (fp16-rounded)
+      float s = 0.f, q = 0.f;
 #pragma unroll
-        for (int j = 0; j < MAXC; ++j) {
-          const int c = cur.c_first + j * EPI_PER_QUAD;
-          if (c >= NCH) break;                       // warp-uniform
-          float f[32];
-          uint32_t a[32], g[32];
-          __syncwarp();
-          tmem_ld32(tquad + acc * BN + c * 32, a);
-          tmem_ld32(tquad + acc * BN + HALF + c * 32, g);
-          tc_wait_ld();
-          const int nv = n0 + c * 32;
-          // packed fp32x2 throughout: folded LayerNorm on value and gate, biases, GELU, product
-          const float2 nm2 = make_float2(nm, nm), rs2 = make_float2(ln.y, ln.y);
-#pragma unroll
-          for (int e = 0; e < 32; e += 4) {
-            float2 a01 = make_float2(__uint_as_float(a[e]), __uint_as_float(a[e + 1])), a23 = make_float2(__uint_as_float(a[e + 2]), __uint_as_float(a[e + 3]));
-            float2 g01 = make_float2(__uint_as_float(g[e]), __uint_as_float(g[e + 1])), g23 = make_float2(__uint_as_float(g[e + 2]), __uint_as_float(g[e + 3]));
-            if (p.ln_stats) {
-              const float4 ca = __ldg(reinterpret_cast<const float4*>(p.ln_colsum + nv + e));
-              const float4 cg = __ldg(reinterpret_cast<const float4*>(p.ln_colsum + nv + HALF + e));
-              a01 = __fmul2_rn(__ffma2_rn(nm2, make_float2(ca.x, ca.y), a01), rs2);
-              a23 = __fmul2_rn(__ffma2_rn(nm2, make_float2(ca.z, ca.w), a23), rs2);
-              g01 = __fmul2_rn(__ffma2_rn(nm2, make_float2(cg.x, cg.y), g01), rs2);
-              g23 = __fmul2_rn(__ffma2_rn(nm2, make_float2(cg.z, cg.w), g23), rs2);
-            }
-            if (cur.bias) {
-              const float4 ba = __ldg(reinterpret_cast<const float4*>(cur.bias + nv + e));
-              const float4 bg = __ldg(reinterpret_cast<const float4*>(cur.bias + nv + HALF + e));
-              a01 = __fadd2_rn(a01, make_float2(ba.x, ba.y)); a23 = __fadd2_rn(a23, make_float2(ba.z, ba.w));
-              g01 = __fadd2_rn(g01, make_float2(bg.x, bg.y)); g23 = __fadd2_rn(g23, make_float2(bg.z, bg.w));
-            }
-            const float2 r01 = __fmul2_rn(a01, gelu_epilogue2(g01)), r23 = __fmul2_rn(a23, gelu_epilogue2(g23));
-            f[e] = r01.x; f[e + 1] = r01.y; f[e + 2] = r23.x; f[e + 3] = r23.y;
-          }
-          epi_store32(p, cur, cur.n_tile * HALF + c * 32, p.N / 2, f, false, stage, lane);
-        }
+      for (int e = 0; e < 32; e += 2) {
+        const float2 r = __half22float2(__floats2half2_rn(f[e], f[e + 1]));
+        s += r.x + r.y;
+        q = fmaf(r.x, r.x, fmaf(r.y, r.y, q));
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) epi_release_acc<PAIR>(&tmem_empty_bar[acc]);
-      if (++acc == NACC) { acc = 0; aph ^= 1; }
+      if (t.row_ok) p.ln_part[(long long)(nb >> 5) * p.ln_rows + t.orow] = make_float2(s, q);
     }
+    if (p.gn_part) gn_part_accumulate(p, t, nb, f, lane);
   }
-  if (p.out_tma && lane == 0) tma_store_wait_all();   // bulk stores must be complete before the CTA exits
+  epi_store32(p, t, col0, n_out, f, !plain && p.res != nullptr && !res_vec, stage, lane);
 }
 #endif  // __CUDACC__
-
-int launch_gemm_pair(int BN, const GemmParams& p, cudaStream_t stream);
 
 }  // namespace vc

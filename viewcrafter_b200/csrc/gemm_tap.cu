@@ -1,4 +1,4 @@
-// Tap-GEMM on tcgen05: D[M,N] = sum_taps A_tap[M,K] * W_tap[N,K]^T  (fp16 in, fp32 accumulate in TMEM).
+// Tap-GEMM on wgmma: D[M,N] = sum_taps A_tap[M,K] * W_tap[N,K]^T  (fp16 in, fp32 accumulate in registers).
 //
 // One kernel family covers every tensor-core op on the U-Net / VAE path:
 //   * nn.Linear / 1x1 conv            : 1 tap, A = [M,K] row-major
@@ -8,18 +8,15 @@
 // A may come from two tensors split along K (channel concat of skip connections without materialising it).
 // Epilogue: + bias[z/bias_z_div][n], GEGLU (value*gelu(gate)), + residual, fp16 / fp32 store (gemm_common.cuh).
 //
-// This file: the host entry point and the ONE-CTA-per-tile persistent kernel (64 + 32 * EPI_WARPS = 448 threads):
-//   warp 0       TMA producer: walks this CTA's tiles and their (tap, k-block) iterations through a smem ring without
-//                draining between tiles, so the loads of tile i+1 are in flight while tile i is still being multiplied
-//   warp 1       TMEM allocator + single-thread tcgen05.mma issuer; TWO accumulators in TMEM (double buffer), so the
-//                main loop of tile i+1 overlaps the epilogue of tile i
-//   warps 2..    epilogue (gemm_epilogue_loop, gemm_common.cuh)
-// Tiles are ordered n-fastest so CTAs that run concurrently share A tiles in L2.  Large problems are routed to the
-// CTA-pair kernel of gemm_tap2.cu (UMMA M=256), which halves the per-SM shared-memory traffic for B.
-#include <cstdlib>
-
+// Persistent kernel, one CTA per SM, 128 x BN tiles, 384 threads:
+//   warpgroup 0  warp 0 is the TMA producer: it walks this CTA's tiles and their (tap, k-block) iterations through a smem
+//                ring without draining between tiles, so the loads of tile i+1 are in flight during the epilogue of tile i
+//   warpgroups 1, 2  wgmma m64nBNk16 on rows [0, 64) / [64, 128) of the tile (both operands from the 128B-swizzled ring),
+//                one k-block in flight behind the one being issued; then the epilogue of their 64 rows
+// Tiles are ordered n-fastest so CTAs that run concurrently share A tiles in L2.
 #include "gemm_common.cuh"
 #include "kernels.h"
+#include "wgmma.cuh"
 
 namespace vc {
 
@@ -28,16 +25,47 @@ struct GemmCfg {
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int BUDGET = 227 * 1024 - 1024 /*align slack*/ - 512 /*barriers*/ - EPI_SMEM_BYTES /*store staging*/;
+  static constexpr int BUDGET = 227 * 1024 - 1024 /*align slack*/ - 256 /*barriers*/ - EPI_SMEM_BYTES;
   static constexpr int STAGES = BUDGET / STAGE_BYTES > 8 ? 8 : BUDGET / STAGE_BYTES;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_SMEM_BYTES + 1024 + 512;
-  // as many accumulators as fit the 512 TMEM columns (2..4): short-K tiles finish their main loop faster than the
-  // accumulator hand-off (commit -> epilogue wake-up -> drain -> arrive) can turn around, so two buffers are not enough
-  static constexpr int NACC = (512 / BN) > 4 ? 4 : (512 / BN);
-  static constexpr int TMEM_COLS = NACC * BN <= 32 ? 32 : NACC * BN <= 64 ? 64 : NACC * BN <= 128 ? 128 : NACC * BN <= 256 ? 256 : 512;
-  static_assert(NACC >= 2 && NACC * BN <= 512, "at least two accumulators must fit TMEM");
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_SMEM_BYTES + 1024 + 256;
   static_assert(STAGES >= 4, "pipeline too shallow");
+  static_assert(B_BYTES % 1024 == 0, "stages must stay 1024-byte aligned (128B swizzle atoms)");
 };
+
+// Drain the accumulator fragments of one MMA warpgroup (64 rows x NCOLS columns) through the transpose buffer, 64 columns at
+// a time, and run the per-chunk epilogue with one row per thread: warp wl of the warpgroup takes rows (wl & 1) * 32 + lane
+// and chunk (wl >> 1) of each 64-column slab.
+template <int BN, int NCOLS>
+__device__ __forceinline__ void epi_drain(const GemmParams& p, const EpiTile& t, float (&acc)[BN / 2], float* xpose, int cw, int wl, int lane,
+                                          uint8_t* stage, bool plain, int nb0, int col0, int n_out) {
+  constexpr int SLABS = (NCOLS + 63) / 64;
+  const int fr = 16 * wl + (lane >> 2), fc = 2 * (lane & 3);   // fragment row / column of d[j * 4] (wgmma accumulator layout)
+#pragma unroll
+  for (int sl = 0; sl < SLABS; ++sl) {
+    named_bar_sync(1 + cw, 128);                   // the previous slab has been read back
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const int j = sl * 8 + jj;
+      if (j < NCOLS / 8) {
+        float* d0 = xpose + fr * EPI_XPOSE_PITCH + jj * 8 + fc;
+        *reinterpret_cast<float2*>(d0) = make_float2(acc[j * 4], acc[j * 4 + 1]);
+        *reinterpret_cast<float2*>(d0 + 8 * EPI_XPOSE_PITCH) = make_float2(acc[j * 4 + 2], acc[j * 4 + 3]);
+      }
+    }
+    named_bar_sync(1 + cw, 128);
+    const int c = sl * 2 + (wl >> 1);
+    if (c * 32 < NCOLS && (plain ? col0 + c * 32 < n_out : nb0 + c * 32 < p.N)) {   // warp-uniform
+      float f[32];
+      const float4* src = reinterpret_cast<const float4*>(xpose + ((wl & 1) * 32 + lane) * EPI_XPOSE_PITCH + (wl >> 1) * 32);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const float4 v = src[e];
+        f[4 * e] = v.x; f[4 * e + 1] = v.y; f[4 * e + 2] = v.z; f[4 * e + 3] = v.w;
+      }
+      epi_chunk(p, t, nb0 + c * 32, col0 + c * 32, n_out, plain, f, stage, lane);
+    }
+  }
+}
 
 template <int BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tap_kernel(const __grid_constant__ GemmParams p) {
@@ -45,50 +73,31 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tap_kernel(const __grid_
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* epi_smem = smem + STAGES * Cfg::STAGE_BYTES;          // per-warp staging tiles of the TMA-store epilogue
+  uint8_t* epi_smem = smem + STAGES * Cfg::STAGE_BYTES;          // [EPI_WARPS] TMA-store staging tiles, [MMA_WGS] transpose buffers
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi_smem + EPI_SMEM_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;     // [NACC]
-  uint64_t* tmem_empty_bar = tmem_full_bar + Cfg::NACC;   // [NACC]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty_bar + Cfg::NACC);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int kblocks = (p.K + BK - 1) / BK;
   const int iters = p.num_taps * kblocks;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.tmap_a);
     tma_prefetch_desc(&p.tmap_b);
     if (p.out_tma) tma_prefetch_desc(&p.tmap_out);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int a = 0; a < Cfg::NACC; ++a) {
-      mbar_init(&tmem_full_bar[a], 1);
-      mbar_init(&tmem_empty_bar[a], EPI_WARPS);
+      mbar_init(&empty_bar[s], EPI_WARPS);          // one arrival per MMA warp
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  // Ring / accumulator positions are carried as (index, phase bit) pairs and tile coordinates come from multiply-high
-  // divisions: the role loops below are single-warp instruction streams whose length bounds the tile rate of short-K
-  // problems (measured: with 64-bit `it % STAGES` arithmetic and generic divisions the empty skeleton -- no TMA, no MMA,
-  // no epilogue -- already cost 1.3 us per tile).
+  // ring positions are carried as (index, phase bit) pairs and tile coordinates come from multiply-high divisions
   if (warp == 0) {
     // ------------------------------ TMA producer ------------------------------
-    // The whole warp runs the loop with warp-uniform control flow and ONE elected lane issues: the compiler can then
-    // keep barrier / descriptor operands in uniform registers (a divergent `if (lane == 0)` loop costs an ELECT/BRA.ANY
-    // serialisation loop around every UTMALDG -- measured).
+    // warp-uniform loop, ONE elected lane issues (keeps barrier / descriptor operands in uniform registers)
     int s = 0;
     uint32_t ph = 0;
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
@@ -103,72 +112,94 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tap_kernel(const __grid_
           if (elect_one()) {
             uint8_t* sa = smem + s * Cfg::STAGE_BYTES;
             uint8_t* sb = sa + Cfg::A_BYTES;
-            if (VC_GEMM_DBG(p, 2)) {
-              mbar_arrive(&full_bar[s]);
-            } else {
-              mbar_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
-              const int k = kb * BK;
-              if (k < p.K1)
-                tma_load_4d(sa, &p.tmap_a, &full_bar[s], k, cx, cy, tc.z);
-              else
-                tma_load_4d(sa, &p.tmap_a2, &full_bar[s], k - p.K1, cx, cy, tc.z);
-              tma_load_2d(sb, &p.tmap_b, &full_bar[s], k, brow);
-            }
+            mbar_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
+            const int k = kb * BK;
+            if (k < p.K1)
+              tma_load_4d(sa, &p.tmap_a, &full_bar[s], k, cx, cy, tc.z);
+            else
+              tma_load_4d(sa, &p.tmap_a2, &full_bar[s], k - p.K1, cx, cy, tc.z);
+            tma_load_2d(sb, &p.tmap_b, &full_bar[s], k, brow);
           }
           __syncwarp();
           if (++s == STAGES) { s = 0; ph ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer ------------------------------
-    // warp-uniform loop, one elected lane issues (always the same lane: tcgen05.commit tracks the issuing thread's MMAs)
-    constexpr uint32_t idesc = umma_idesc_f16(BM, BN);
-    // smem descriptors: only the 14-bit start-address field (bytes >> 4) changes between stages / k-slices and the ring
-    // lies below 256 KB, so the field never carries: descriptors are formed by integer adds on the low word
-    const uint64_t desc0 = umma_desc_sw128(smem_u32(smem));
-    const uint32_t desc_hi = (uint32_t)(desc0 >> 32), desc_lo = (uint32_t)desc0;
-    int s = 0, acc = 0;
-    uint32_t ph = 0, aph = 0;
+  } else if (warp >= 4) {
+    // ------------------------------ MMA warpgroups + epilogue ------------------------------
+    const int cw = (warp >> 2) - 1;                 // rows [64 cw, 64 cw + 64) of every tile
+    const int wl = warp & 3;
+    uint8_t* stage = epi_smem + (warp - 4) * EPI_STAGE_BYTES;
+    float* xpose = reinterpret_cast<float*>(epi_smem + EPI_WARPS * EPI_STAGE_BYTES + cw * EPI_XPOSE_BYTES);
+    const uint32_t ring = smem_u32(smem);
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int s = 0;
+    uint32_t ph = 0;
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      mbar_wait(&tmem_empty_bar[acc], aph ^ 1);    // the epilogue must have drained this accumulator
-      tc_fence_after();
-      const uint32_t tacc = tmem_base + acc * BN;
+      int prev = -1;
       for (int i = 0; i < iters; ++i) {
         mbar_wait(&full_bar[s], ph);
-        tc_fence_after();
-        if (elect_one()) {
-          if (VC_GEMM_DBG(p, 1)) {
-            mbar_arrive(&empty_bar[s]);
-          } else {
-            const uint32_t la = desc_lo + (uint32_t)(s * (Cfg::STAGE_BYTES >> 4));
+        const uint32_t a_addr = ring + s * Cfg::STAGE_BYTES + cw * (64 * BK * 2);
+        const uint32_t b_addr = ring + s * Cfg::STAGE_BYTES + Cfg::A_BYTES;
+        wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < BK / 16; ++k)
-              umma_ss(tacc, ((uint64_t)desc_hi << 32) | (la + 2 * k), ((uint64_t)desc_hi << 32) | (la + (Cfg::A_BYTES >> 4) + 2 * k), idesc,
-                      (i > 0 || k > 0) ? 1u : 0u);
-            umma_commit(&empty_bar[s]);   // frees the smem stage once these MMAs have read it
-          }
+        for (int k = 0; k < BK / 16; ++k)
+          Wgmma<BN>::ss(acc, wgmma_desc_sw128(a_addr + 32 * k), wgmma_desc_sw128(b_addr + 32 * k), (i > 0 || k > 0) ? 1 : 0);
+        wgmma_commit();
+        wgmma_wait<1>();                            // the previous k-block's MMAs have retired: its stage may be refilled
+        if (prev >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);
         }
-        __syncwarp();
+        prev = s;
         if (++s == STAGES) { s = 0; ph ^= 1; }
       }
-      if (elect_one()) {
-        if (VC_GEMM_DBG(p, 1)) mbar_arrive(&tmem_full_bar[acc]);
-        else umma_commit(&tmem_full_bar[acc]);   // accumulator complete
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
       }
-      __syncwarp();
-      if (++acc == Cfg::NACC) { acc = 0; aph ^= 1; }
+      const EpiTile t = epi_tile(p, tile, cw * 2 + (wl & 1), lane);
+      const int n0 = t.n_tile * BN;
+      if (!p.geglu) {
+        epi_drain<BN, BN>(p, t, acc, xpose, cw, wl, lane, stage, false, n0, n0, p.N);
+      } else {
+        // GEGLU on the fragments: tile columns [0, BN/2) are values, [BN/2, BN) the matching gates (weights were interleaved
+        // per tile); out[:, n_tile*BN/2 + c] = (value + bias_v) * gelu(gate + bias_g).  No residual (checked on the host).
+        constexpr int HALF = BN / 2;
+        const TileCoord tc = tile_coord_m(p, t.m_tile);
+        float2 ln[2] = {make_float2(0.f, 1.f), make_float2(0.f, 1.f)};
+        if (p.ln_stats) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int R = cw * 64 + 16 * wl + (lane >> 2) + 8 * h;
+            const int x = tc.x0 + (R & (p.bx - 1)), y = tc.y0 + (R >> p.bx_shift);
+            if (x < p.X && y < p.Y && tc.z < p.Z)
+              ln[h] = __ldg(reinterpret_cast<const float2*>(p.ln_stats) + ((long long)tc.z * p.Y + y) * p.X + x);
+          }
+        }
+#pragma unroll
+        for (int j = 0; j < HALF / 8; ++j) {
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int n = n0 + 8 * j + 2 * (lane & 3) + (e & 1);
+            float a = acc[j * 4 + e], g = acc[(j + HALF / 8) * 4 + e];
+            if (p.ln_stats) {
+              const float2 l = ln[e >> 1];
+              a = (a - l.x * __ldg(p.ln_colsum + n)) * l.y;
+              g = (g - l.x * __ldg(p.ln_colsum + n + HALF)) * l.y;
+            }
+            if (t.bias) { a += __ldg(t.bias + n); g += __ldg(t.bias + n + HALF); }
+            acc[j * 4 + e] = a * gelu_epilogue(g);
+          }
+        }
+        epi_drain<BN, HALF>(p, t, acc, xpose, cw, wl, lane, stage, true, n0, t.n_tile * HALF, p.N / 2);
+      }
     }
-  } else {
-    // ------------------------------ epilogue ------------------------------
-    gemm_epilogue_loop<BN, Cfg::NACC, false>(p, blockIdx.x, gridDim.x, 1, 0, tmem_base, tmem_full_bar, tmem_empty_bar, epi_smem, warp, lane);
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+    if (p.out_tma && lane == 0) tma_store_wait_all();   // bulk stores must be complete before the CTA exits
   }
 }
 
@@ -186,15 +217,11 @@ static int launch_gemm(const GemmParams& p, cudaStream_t stream) {
   return VC_OK;
 }
 
+// Widest tile that divides N: the accumulator lives in registers (BN / 2 per MMA thread), so tiles stop at 160 columns.
 static int pick_bn(int N, int geglu) {
-  if (geglu) {
-    static int g = -1;                       // tuning switch VC_GEGLU_BN=128|256
-    if (g < 0) { const char* e = getenv("VC_GEGLU_BN"); g = e ? atoi(e) : 256; }
-    return (g == 256 && N % 256 == 0) ? 256 : 128;
-  }
+  if (geglu) return 128;
   if (N <= 32) return 32;
   if (N <= 64) return 64;
-  if (N % 256 == 0) return 256;
   if (N % 160 == 0) return 160;
   if (N % 128 == 0) return 128;
   if (N % 96 == 0 && N <= 192) return 96;
@@ -203,16 +230,6 @@ static int pick_bn(int N, int geglu) {
 }
 
 int pick_bn_public(int N, int geglu) { return pick_bn(N, geglu); }
-
-// tuning switch: VC_GEMM_PAIR=0 forces the one-CTA kernel everywhere, =1 (default) uses CTA pairs for large problems
-static int pair_mode() {
-  static int mode = -1;
-  if (mode < 0) {
-    const char* e = getenv("VC_GEMM_PAIR");
-    mode = (e && e[0] == '0') ? 0 : 1;
-  }
-  return mode;
-}
 
 int gemm_tap(const GemmDesc& d, cudaStream_t stream) {
   VC_REQUIRE(d.a && d.w && (d.out || d.out_f32), "gemm_tap: null pointer");
@@ -231,49 +248,7 @@ int gemm_tap(const GemmDesc& d, cudaStream_t stream) {
 
   GemmParams p;
   memset(&p, 0, sizeof(p));
-  int BN = pick_bn(d.N, d.geglu);
-  int tuned = 0;                              // 0: default pair rule; 1: tuned -> CTA pairs; 2: tuned -> single CTAs
-  {
-    // Wave quantisation: the persistent grid runs ceil(tiles / slots) rounds.  A frame shard of a multi-GPU run (7 frames at
-    // 18x32: 32 row tiles x 1280 columns) gives 80 pair tiles on 74 SM pairs -- two rounds, the second 8 % full.  When the default
-    // tiling fills its rounds to less than 80 %, compare (pair | single CTA) x (BN 256 | 160 | 128) by
-    // rounds x tile area / relative tile efficiency and take the cheapest.  GEGLU keeps the tile its weights were interleaved for.
-    static int tune = -1;                     // tuning switch VC_GEMM_WAVE_TUNE=0 keeps the fixed choice
-    if (tune < 0) { const char* e = getenv("VC_GEMM_WAVE_TUNE"); tune = (e && e[0] == '0') ? 0 : 1; }
-    const long long mt = (long long)((d.X + d.bx - 1) / d.bx) * ((d.Y + d.by - 1) / d.by) * d.Z;
-    const int k_it = d.num_taps * ((d.K + BK - 1) / BK);
-    const int sms = sm_count();
-    auto cost = [&](int bn, bool pair, double* fill) -> double {
-      const long long nt = (d.N + bn - 1) / bn;
-      const long long tiles = (pair ? (mt + 1) / 2 : mt) * nt;
-      const long long slots = pair ? sms / 2 : sms;
-      const long long rounds = (tiles + slots - 1) / slots;
-      if (fill) *fill = (double)tiles / (double)(rounds * slots);
-      const double eff = (pair ? 1.08 : 1.0) * (bn == 256 ? 1.0 : bn == 160 ? 0.97 : 0.94);
-      return (double)rounds * (pair ? 2.0 : 1.0) * bn / eff;
-    };
-    auto pair_ok = [&](int bn) { return pair_mode() && d.N % bn == 0 && k_it >= 5 && (mt / 2) * ((d.N + bn - 1) / bn) >= 1; };
-    if (tune && !d.geglu && d.N >= 128 && (BN == 256 || BN == 160 || BN == 128)) {
-      double fill = 1.0;
-      const bool def_pair = pair_ok(BN) && (mt / 2) * ((d.N + BN - 1) / BN) >= sms;
-      double best = cost(BN, def_pair, &fill);
-      if (fill < 0.8) {
-        int best_bn = BN; bool best_pair = def_pair;
-        const int cands[3] = {256, 160, 128};
-        for (int ci = 0; ci < 3; ++ci) {
-          const int bn = cands[ci];
-          if (d.N % bn != 0) continue;
-          for (int pr = 0; pr < 2; ++pr) {
-            if (pr && !pair_ok(bn)) continue;
-            const double c = cost(bn, pr != 0, nullptr);
-            if (c < best * 0.97) { best = c; best_bn = bn; best_pair = pr != 0; }
-          }
-        }
-        BN = best_bn;
-        tuned = best_pair ? 1 : 2;
-      }
-    }
-  }
+  const int BN = pick_bn(d.N, d.geglu);
   p.bx = d.bx; p.by = d.by; p.X = d.X; p.Y = d.Y; p.Z = d.Z;
   p.tiles_x = (d.X + d.bx - 1) / d.bx;
   p.tiles_y = (d.Y + d.by - 1) / d.by;
@@ -285,17 +260,6 @@ int gemm_tap(const GemmDesc& d, cudaStream_t stream) {
   while ((1 << p.bx_shift) < d.bx) ++p.bx_shift;
   VC_REQUIRE((1 << p.bx_shift) == d.bx, "gemm_tap: bx=%d must be a power of two", d.bx);
   const long long m_tiles = (long long)p.tiles_x * p.tiles_y * p.Z;
-  // CTA pairs pay off once every SM pair has several 256-row tiles; N must be covered by whole BN tiles so that each
-  // CTA's half of the B tile (BN/2 rows) never straddles a tap boundary
-  // Measured on B200 (profiles/README.md): pairs win 10-15 % on long reductions; since the role loops were slimmed down they
-  // also win 4-13 % on the short-K (K = 320 / 512, 5-8 k-blocks) level-0 linears (they lost there before).
-  const int k_iters = d.num_taps * ((d.K + BK - 1) / BK);
-  static int pair_min_k = -1;                  // tuning switch VC_GEMM_PAIR_MINK: shortest reduction (in 64-wide k-blocks) routed to CTA pairs
-  if (pair_min_k < 0) { const char* e = getenv("VC_GEMM_PAIR_MINK"); pair_min_k = e ? atoi(e) : 5; }
-  // default rule: pairs once every SM pair has work; a wave-tuned choice (above) decides by its cost model instead
-  const bool use_pair = tuned == 1 ? true : tuned == 2 ? false :
-                        (pair_mode() && (BN == 128 || BN == 160 || BN == 256) && d.N % BN == 0 && k_iters >= pair_min_k &&
-                         (m_tiles / 2) * p.n_tiles >= sm_count());
 
   // A: (K, X, Y, Z) with row pitch lda
   {
@@ -316,7 +280,7 @@ int gemm_tap(const GemmDesc& d, cudaStream_t stream) {
   {
     uint64_t dims[2] = {(uint64_t)d.K, (uint64_t)d.num_taps * d.N};
     uint64_t str[1] = {(uint64_t)(d.ldw > 0 ? d.ldw : d.K) * 2};
-    uint32_t box[2] = {(uint32_t)BK, (uint32_t)(use_pair ? BN / 2 : BN)};
+    uint32_t box[2] = {(uint32_t)BK, (uint32_t)BN};
     int rc = encode_tmap_f16(&p.tmap_b, d.w, 2, dims, str, box);
     if (rc) return rc;
   }
@@ -341,17 +305,15 @@ int gemm_tap(const GemmDesc& d, cudaStream_t stream) {
                             (reinterpret_cast<uintptr_t>(d.gn_part) & 7) == 0),
              "gemm_tap: GroupNorm partial sums need an fp16 output with N %% 32 == 0 and N %% gn_sub == 0 (gn_sub 10 or 8)");
   p.gn_part = reinterpret_cast<float2*>(d.gn_part); p.gn_hp = d.gn_sub / 2; p.gn_nchunks = d.N / 32;
-  // 256-bit epilogue accesses need 32-byte aligned rows (true for every activation on the U-Net / VAE path); anything
+  // vector epilogue accesses need 32-byte aligned rows (true for every activation on the U-Net / VAE path); anything
   // else (odd pitches, the 4- and 3-channel output convs) takes the predicated scalar path inside the kernel
   const bool o_al = ((reinterpret_cast<uintptr_t>(optr) & 31) == 0) && ((long long)d.ldo * esz) % 32 == 0;
   const bool r_al = !d.res || (((reinterpret_cast<uintptr_t>(d.res) & 31) == 0) && ((long long)d.ldr * 2) % 32 == 0);
   p.vec_ok = (o_al && r_al) ? 1 : 0;
   {
     // TMA-store epilogue: fp16 output whose width is whole 32-column chunks and whose rows are 16-byte aligned
-    static int tma_store = -1;                 // tuning switch VC_GEMM_TMA_STORE=0 keeps the direct-store epilogue
-    if (tma_store < 0) { const char* e = getenv("VC_GEMM_TMA_STORE"); tma_store = (e && e[0] == '0') ? 0 : 1; }
     const int n_out = d.geglu ? d.N / 2 : d.N;
-    p.out_tma = (tma_store && d.out && !d.out_f32 && n_out % 32 == 0 && (reinterpret_cast<uintptr_t>(d.out) & 15) == 0 && d.ldo % 8 == 0) ? 1 : 0;
+    p.out_tma = (d.out && !d.out_f32 && n_out % 32 == 0 && (reinterpret_cast<uintptr_t>(d.out) & 15) == 0 && d.ldo % 8 == 0) ? 1 : 0;
     if (p.out_tma) {
       const uint32_t bw = d.bx < 32 ? d.bx : 32;
       uint64_t dims[4] = {(uint64_t)n_out, (uint64_t)d.X, (uint64_t)d.Y, (uint64_t)d.Z};
@@ -398,25 +360,15 @@ int gemm_tap(const GemmDesc& d, cudaStream_t stream) {
       if (rc) return rc;
     }
   }
-  {
-    static int dbg = -1;
-    if (dbg < 0) {
-      const char* e = getenv("VC_GEMM_DEBUG");
-      dbg = e ? atoi(e) : 0;
-    }
-    p.debug = dbg;
-  }
-  const long long total = (use_pair ? (m_tiles + 1) / 2 : m_tiles) * p.n_tiles;
+  const long long total = m_tiles * p.n_tiles;
   VC_REQUIRE(total > 0 && total < (1ll << 31), "gemm_tap: tile count %lld out of range", total);
   p.total_tiles = (int)total;
-  if (use_pair) return launch_gemm_pair(BN, p, stream);
   switch (BN) {
     case 32: return launch_gemm<32>(p, stream);
     case 64: return launch_gemm<64>(p, stream);
     case 96: return launch_gemm<96>(p, stream);
     case 128: return launch_gemm<128>(p, stream);
     case 160: return launch_gemm<160>(p, stream);
-    case 256: return launch_gemm<256>(p, stream);
   }
   set_error("gemm_tap: no kernel for BN=%d", BN);
   return VC_ERR_UNSUPPORTED;

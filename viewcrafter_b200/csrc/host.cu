@@ -22,11 +22,11 @@ const char* last_error() { return g_err; }
 int sm_count() {
   static std::atomic<int> cache[256];
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   const int slot = dev & 255;
   int n = cache[slot].load(std::memory_order_relaxed);
   if (n == 0) {
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cache[slot].store(n, std::memory_order_relaxed);
   }
   return n;

@@ -1,4 +1,4 @@
-// Internal C++ launch interface of the sm_100a kernels (the public boundary is include/vc_b200.h).
+// Internal C++ launch interface of the sm_90a kernels (the public boundary is include/vc_b200.h).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -43,7 +43,7 @@ struct GemmDesc {
   // columns [n, n + 32) of the row, of the fp16-rounded values; layernorm_stats_from_parts turns them into (mean, rstd)
   float* ln_part = nullptr;
   // GroupNorm statistics of the OUTPUT, gathered in the epilogue (gemm_common.cuh: gn_part_accumulate): per 32-row block
-  // rb = m_tile * 4 + quadrant (m-tiles in x, y, z order; CTA pairs pad the m-tile count to an even number), 32-column chunk and piece,
+  // rb = m_tile * 4 + quadrant (m-tiles in x, y, z order), 32-column chunk and piece,
   // gn_part[((rb * (N / 32) + chunk) * 4 + piece) * 2] = (sum, sumsq) of the fp16-rounded outputs; chunks are cut at multiples of
   // gn_sub channels (10 or 8).  groupnorm_from_parts() turns them into per-group statistics and normalises in ONE pass.
   float* gn_part = nullptr;
@@ -64,10 +64,6 @@ struct AttnDesc {
   int accumulate = 0;              // out += result (second softmax branch of the image cross-attention)
 };
 int flash_attn_d64(const AttnDesc& d, cudaStream_t stream);
-// 64-key-tile / 3-CTAs-per-SM variant (attention_bn64.cu): flash_attn_d64 forwards short key sequences (Nk <= 1024) to it;
-// env VC_ATTN_BN64 = 1 / 0 forces / forbids it (mode: 1, 0, or -1 = by size)
-int flash_attn_bn64_mode();
-int flash_attn_d64_bn64(const AttnDesc& d, cudaStream_t stream);
 
 // GroupNorm(32) on NHWC fp16; x is the channel concat of (x1: C1 channels) and (x2: C2 channels, may be null).
 // Statistics over `rows_per_sample` rows (pixels, or frames*pixels for the 5-D variant) x C/32 channels.

@@ -104,8 +104,7 @@ __device__ __forceinline__ void gn_stats_dev(const __half* __restrict__ x1, cons
 #define VC_SILU_TANH 1       // A/B switch: SiLU through ONE MUFU op (tanh.approx) instead of ex2 + rcp
 #endif
 // x * sigmoid(x) = h + h * tanh(h) with h = x / 2: one MUFU.TANH + 2 FP ops per element instead of MUFU.EX2 + MUFU.RCP + 3.  The
-// normalise pass issues 2 MUFU per element otherwise and is then bound by the 16-per-clock MUFU pipe (41 us for the 74 M elements of
-// a 25x72x128x320 tensor) rather than by HBM.  tanh.approx.f32 has a relative error of 2^-11 on tanh, i.e. an absolute error of
+// normalise pass issues 2 MUFU per element otherwise and is then bound by the 16-per-clock MUFU pipe rather than by HBM.  tanh.approx.f32 has a relative error of 2^-11 on tanh, i.e. an absolute error of
 // <= 2.4e-4 |x| on the result -- the size of the fp16 rounding the output gets anyway.
 __device__ __forceinline__ float gn_silu(float x) {
 #if VC_SILU_TANH
@@ -171,8 +170,8 @@ __device__ __forceinline__ void gn_apply_dev(const __half* __restrict__ x1, cons
   const GnThread t = gn_thread(x1, x2, g, split, sample, v, pl);
   const long long ostride = (long long)g.ppi * g.C;
   // Walk the rows BACKWARDS (VC_GN_REVERSE): in the fused kernel the statistics pass streamed them forwards, so what the L2 still
-  // holds is the tail of every CTA's slice; a second forward sweep is the worst case for an LRU-like cache (ncu, C=320 @25x72x128:
-  // L2 hit 0.4 %, 294 MB read from DRAM for a 147 MB tensor), the reverse sweep meets the resident lines first.
+  // holds is the tail of every CTA's slice; a second forward sweep is the worst case for an LRU-like cache, the reverse sweep meets
+  // the resident lines first.
   // Software pipeline: the loads of the NEXT four rows are issued before the current four are normalised and stored, so up to eight
   // 16-byte loads per thread are in flight and the DRAM latency is covered when this pass is the only one (statistics from the
   // producing GEMM: no L2-resident tail to meet).
@@ -212,8 +211,8 @@ __global__ void __launch_bounds__(512, 2) gn_apply_kernel(const __half* __restri
   gn_apply_dev(x1, x2, g, partial, gamma, beta, eps, silu, out, blockIdx.x, blockIdx.y);
 }
 // Fused single launch: statistics pass, a grid-wide rendezvous of the CTAs of one sample (all CTAs are co-resident by
-// construction -- the host checks the occupancy), then the normalise pass, whose re-read of x is served by the 126 MB L2
-// for everything but the largest 5-D tensors: HBM traffic drops from 3 passes to ~2.
+// construction -- the host checks the occupancy), then the normalise pass, whose re-read of x is served by the L2 (50 MB
+// on H100) when a sample fits it: HBM traffic drops from 3 passes to ~2.
 __global__ void __launch_bounds__(512, 2) gn_fused_kernel(const __half* __restrict__ x1, const __half* __restrict__ x2, GnGeom g,
                                                         float* __restrict__ partial, unsigned int* __restrict__ counters,
                                                         const float* __restrict__ gamma, const float* __restrict__ beta, float eps, int silu,
@@ -270,9 +269,6 @@ int groupnorm_nhwc(const __half* x1, int C1, const __half* x2, int C2, int sampl
   // fused path: the statistics -> normalise hand-over is a grid-wide rendezvous, so every CTA must be resident at once.
   // The launch is COOPERATIVE: the driver either co-schedules the whole grid or refuses the launch -- it cannot hang when
   // other work holds SMs (the occupancy figure only sizes the grid).
-  // Measured alternatives that did NOT pay off (profiles/README.md, round 2): launching the samples in L2-sized chunks and a
-  // team-pipelined persistent kernel -- both make the re-read an L2 hit, both were 20-45 % slower than this single launch
-  // (shorter phases, more rendezvous); the lever left is to take the statistics from the producing GEMM's epilogue.
   const size_t part_bytes = (size_t)samples * g.splits * 64 * sizeof(float);
   int per_sm = 0;
   VC_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gn_fused_kernel, threads, smem));
@@ -589,7 +585,7 @@ int layernorm_rows(const __half* x, long long rows, int C, const float* gamma, c
 // epilogue (GemmDesc::ln_stats), which turns LayerNorm from a read + write pass into this read-only pass.
 // One warp per group of 4 rows, every lane keeps 4 independent 16-byte loads in flight; sums are taken about a per-row
 // pivot (the row's first element) so the one-pass variance does not cancel when |mean| >> std.  ~40 registers: 48+ warps
-// per SM (the register-resident two-pass kernel above runs at 16 warps per SM and ~2.6 TB/s as a pure reader).
+// per SM (the register-resident two-pass kernel above runs at 16 warps per SM).
 __global__ void __launch_bounds__(256) ln_stats_kernel(const __half* __restrict__ x, long long rows, int C, float eps,
                                                        float2* __restrict__ stats) {
   const int lane = threadIdx.x & 31;
@@ -644,8 +640,7 @@ __global__ void __launch_bounds__(256) ln_stats_kernel(const __half* __restrict_
 }
 
 // Default for C <= 1024: the same statistics with every 16-byte load of a warp's 4 rows issued before the first conversion
-// (ITERS x 4 loads in flight per lane instead of 4): the rolled loop above read at 2.75 TB/s, this one at 3.95 TB/s (C=320) and
-// 5.5 TB/s (C=512) on the B200 (profiles/r02_ab_micro.txt).  Arithmetic and rounding order per lane are those of
+// (ITERS x 4 loads in flight per lane instead of 4).  Arithmetic and rounding order per lane are those of
 // ln_stats_kernel, so the results are bit-identical.
 template <int ITERS>
 __global__ void __launch_bounds__(256) ln_stats_unrolled_kernel(const __half* __restrict__ x, long long rows, int C, float eps,
@@ -743,7 +738,7 @@ int layernorm_stats(const __half* x, long long rows, int C, float eps, float* st
   long long blocks = (rows + 4 * wpb - 1) / (4 * wpb);
   const long long cap = (long long)sm_count() * 8;              // 8 x 256 threads = 64 warps per SM
   if (blocks > cap) blocks = cap;
-  static int unroll = -1;                       // VC_LN_STATS_UNROLL=0: the rolled loop (measured on B200: 53.6 -> 37.3 us at C=320 x 230400 rows)
+  static int unroll = -1;                       // VC_LN_STATS_UNROLL=0: the rolled loop
   if (unroll < 0) { const char* e = getenv("VC_LN_STATS_UNROLL"); unroll = (e && e[0] == '0') ? 0 : 1; }
   const int iters = (C / 8 + 31) / 32;
   if (unroll && iters <= 2)

@@ -2,7 +2,7 @@
 // lvdm/modules/attention.py:81-126 with N = T, batch = H*W sites; the reference always takes the naive
 // einsum-softmax-einsum path here, attention.py:66).
 //
-// The problem per (site, head) is a 25x25x64 attention: far below the 128-row granularity of a tcgen05 MMA and
+// The problem per (site, head) is a 25x25x64 attention: far below the 64-row granularity of a wgmma and
 // HBM-bound (3 x T x 128 B in, T x 128 B out per pair), so it runs on warp-level mma.sync m16n8k16 tiles: one warp
 // per (site, head), Q/K/V staged in shared memory with 16-byte coalesced loads, S and O accumulators in registers,
 // softmax on the accumulator fragments, P re-used in registers as the A operand of P.V (no smem round trip).

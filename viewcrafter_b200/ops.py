@@ -27,7 +27,7 @@ def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
 def require_cuda(device, who: str):
     """The product has no CPU path: anything not on a CUDA device is an error, not a fallback."""
     if torch.device(device).type != "cuda":
-        raise _lib.VcError(f"{who} runs only on a CUDA (sm_100a) device; there is no CPU path")
+        raise _lib.VcError(f"{who} runs only on a CUDA (sm_90a) device; there is no CPU path")
 
 
 VcError = _lib.VcError
@@ -150,9 +150,10 @@ LN_FROM_PRODUCER = os.environ.get("VC_LN_FROM_PRODUCER", "1") != "0"   # A/B swi
 GN_FROM_PRODUCER = int(os.environ.get("VC_GN_FROM_PRODUCER", "1"))
 # ... taken for every GroupNorm with <= 4 samples (the 5-D ones: one sample = a whole batch element, so the fused kernel's statistics and
 # normalise phases cannot overlap across samples) and for per-frame GroupNorms of at least this many MB; smaller per-frame tensors are re-read
-# from the 126 MB L2 by the one-launch fused kernel, which then beats finalize + normalise (measured on B200, profiles/README.md round 2:
-# 5-D 75 vs 97 us at level 0, 46 vs 59 at level 1, 33 vs 42 at level 2; 4-D 139 vs 161 us at level 0 B=2, but 51 vs 47 at level 1)
-GN_PARTS_MIN_MB = float(os.environ.get("VC_GN_PARTS_MIN_MB", "100"))
+# from L2 by the one-launch fused kernel.  Measured on an H100 80GB HBM3 at a 400 W power limit (tools/gn_parts_micro.py, per-frame GroupNorm
+# over 50 frames, B = 2): producer sums 283 vs 364 us at 295 MB (level 0), 149 vs 194 at 147 MB, 92 vs 125 at 74 MB, 48 vs 53 at 18 MB
+# (level 3) -- the producer sums win at every U-Net level, so the threshold sits below the smallest one
+GN_PARTS_MIN_MB = float(os.environ.get("VC_GN_PARTS_MIN_MB", "16"))
 GN_SUB = 10          # sub-group width the U-Net producers cut their chunks at: every GroupNorm(32) boundary of 320 / 640 / 1280 channels
                      # and of their skip concats (640 / 960 / 1280 / 1920 / 2560) is a multiple of 10
 
@@ -190,7 +191,7 @@ def _gn_part_alloc(d: GemmDesc, device):
         return None
     tx, ty = -(-d.X // d.bx), -(-d.Y // d.by)
     m_tiles = tx * ty * d.Z
-    n_rb = (m_tiles + 1) // 2 * 2 * 4                           # CTA pairs touch an even number of m-tiles
+    n_rb = m_tiles * 4                                          # one record row per 32-row block
     part = torch.empty((n_rb, N // 32, 4, 2), device=device, dtype=torch.float32)
     d.gn_part, d.gn_sub = part.data_ptr(), GN_SUB
     return GnPart(part, N // 32, GN_SUB, tx * ty * 4, d.X * d.Y, d.Z, linear=(d.by == 1 and d.bx == 128 and (d.Y == 1 or d.X % 128 == 0)))

@@ -175,8 +175,9 @@ class PeerFrameComm(FrameComm):
         # layout switches inside the producing GEMM's epilogue (scatter_plan): "0" off, "1" every supported shape, "aligned" (default) only
         # shapes whose 32-row epilogue patches never straddle a rank's pixel range or a frame (H*W/P and H*W multiples of 32)
         self.fused = os.environ.get("VC_PEER_FUSED", "aligned")
-        # ... and only for frame groups of at most this many ranks: 2 is what was validated on hardware (round 2: probe at the real level shapes,
-        # sharded forward vs single GPU, graph replay, bench); the kernels handle up to 4 ranks (VC_PEER_FUSED_MAXP=4)
+        # ... and only for frame groups of at most this many ranks: 2 is the largest group the fused switches were checked with on
+        # multi-GPU hardware (probe at the real level shapes, sharded forward vs single GPU, graph replay); the kernels handle up to 4
+        # ranks (VC_PEER_FUSED_MAXP=4)
         self.fused_max_p = int(os.environ.get("VC_PEER_FUSED_MAXP", "2"))
         self.fused_switches = 0
 

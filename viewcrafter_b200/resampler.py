@@ -5,7 +5,7 @@
 U-Net's image cross-attention consumes (utils/diffusion_utils.py:128-129,149-150; twice per clip).  Same constructor
 kwargs, ``forward`` signature and state-dict keys (``latents``, ``proj_in``, ``proj_out``, ``norm_out``,
 ``layers.{i}.0.{norm1,norm2,to_q,to_kv,to_out}``, ``layers.{i}.1.{0,1,3}``) as the reference; the forward runs on the
-same CUDA kernels as the U-Net: tcgen05 tap-GEMM for every Linear (residual adds fused into the epilogue), the d=64
+same CUDA kernels as the U-Net: wgmma tap-GEMM for every Linear (residual adds fused into the epilogue), the d=64
 flash-attention kernel for PerceiverAttention (scale = dim_head**-0.25 applied to q and k = dim_head**-0.5 on the
 scores), LayerNorm rows, exact-erf GELU.  No CPU path (ops.require_cuda).
 """

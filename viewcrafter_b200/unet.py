@@ -5,9 +5,9 @@ state-dict keys/shapes (SURVEY.md Appendix B) so the reference checkpoint loads 
 ``torch.nn`` modules below are *parameter holders only*: ``forward`` never calls them.  All arithmetic runs in
 libvc_b200.so on channels-last fp16 activations (``rows = (b t) h w``, columns = channels):
 
-    ResBlock            -> GroupNorm+SiLU kernel, 9-tap tcgen05 GEMM (+emb bias), again, 1x1 skip GEMM fused as
+    ResBlock            -> GroupNorm+SiLU kernel, 9-tap wgmma GEMM (+emb bias), again, 1x1 skip GEMM fused as
                            residual, then 4x [5-D GroupNorm+SiLU, 3-tap temporal GEMM]          (:210-279)
-    SpatialTransformer  -> GroupNorm, proj_in GEMM, LN, fused-QKV GEMM, tcgen05 flash attention, out-proj GEMM
+    SpatialTransformer  -> GroupNorm, proj_in GEMM, LN, fused-QKV GEMM, wgmma flash attention, out-proj GEMM
                            (+res), LN, q GEMM, text + image cross attention (accumulate), LN, GEGLU GEMM, FF GEMM,
                            proj_out GEMM (+x_in)                                                  (attention.py:249-310)
     TemporalTransformer -> same with the temporal (T<=32) attention kernel, no transposes: tokens stay in
