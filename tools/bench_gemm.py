@@ -5,7 +5,7 @@ import torch
 from viewcrafter_b200 import ops
 
 dev = "cuda"
-def t(fn, reps=5):
+def t(fn, reps=20):
     fn(); torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
@@ -46,6 +46,8 @@ lin("linear l0 320->320 +res", M0, 320, 320, res=True)
 lin("qkv l0 320->960", M0, 320, 960, bias=False)
 lin("geglu l0 320->2560", M0, 320, 2560, geglu=True)
 lin("ff2 l0 1280->320 +res", M0, 1280, 320, res=True)
+lin("linear l1 640->640 +res", M1, 640, 640, res=True)
+lin("qkv l1 640->1920", M1, 640, 1920, bias=False)
 lin("geglu l1 640->5120", M1, 640, 5120, geglu=True)
 lin("ff2 l1 2560->640 +res", M1, 2560, 640, res=True)
 lin("qkv l2 1280->3840", M2, 1280, 3840, bias=False)

@@ -148,6 +148,13 @@ __device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
 }
 // named barrier over `count` threads (one id per warpgroup; id 0 is __syncthreads)
 __device__ __forceinline__ void named_bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+// signal a named barrier without waiting for it; `count` covers the arriving and the waiting (named_bar_sync) threads
+__device__ __forceinline__ void named_bar_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+// move registers between the warpgroups of a CTA (warpgroup-collective; the per-SM register file must hold the new split)
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // Shared-memory matrix descriptor, 128B swizzle, rows of 128 bytes (64 fp16) stored densely, as TMA writes them with
 // CU_TENSOR_MAP_SWIZZLE_128B:

@@ -8,9 +8,15 @@ namespace vc {
 static constexpr int BM = 128;
 static constexpr int BK = 64;
 static constexpr int MAX_TAPS = 9;
-// one producer warpgroup (TMA) + two MMA warpgroups, each owning 64 of the tile's 128 rows
+// one producer warpgroup (TMA) + two MMA warpgroups, each owning whole 128-row tiles (alternate tiles of the CTA's sequence)
 static constexpr int MMA_WGS = 2;
 static constexpr int GEMM_THREADS = 128 * (1 + MMA_WGS);
+// Register split (setmaxnreg): the CTA is launched with 168 registers per thread (65536 / 384, rounded down to a multiple of
+// 8); the producer warpgroup hands its share to the MMA warpgroups, whose 2 x BN / 2 accumulators per thread need it.
+static constexpr int GEMM_LAUNCH_REGS = 168;
+static constexpr int GEMM_PRODUCER_REGS = 24;
+static constexpr int GEMM_MMA_REGS = 240;
+static_assert(128 * GEMM_PRODUCER_REGS + 128 * MMA_WGS * GEMM_MMA_REGS <= GEMM_LAUNCH_REGS * GEMM_THREADS, "register split exceeds the CTA's allocation");
 static constexpr int EPI_WARPS = 4 * MMA_WGS;
 static constexpr int EPI_STAGE_BYTES = 32 * 32 * 2;              // one warp's staging tile for TMA stores: 32 rows x 32 fp16
 // accumulator transpose: an MMA warpgroup writes 64 rows x 64 columns of fp32 at a time, then each warp reads back 32 rows x

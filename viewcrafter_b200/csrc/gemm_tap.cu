@@ -8,11 +8,18 @@
 // A may come from two tensors split along K (channel concat of skip connections without materialising it).
 // Epilogue: + bias[z/bias_z_div][n], GEGLU (value*gelu(gate)), + residual, fp16 / fp32 store (gemm_common.cuh).
 //
-// Persistent kernel, one CTA per SM, 128 x BN tiles, 384 threads:
+// Persistent kernel, one CTA per SM, 128 x BN tiles, 384 threads, ping-pong schedule:
 //   warpgroup 0  warp 0 is the TMA producer: it walks this CTA's tiles and their (tap, k-block) iterations through a smem
-//                ring without draining between tiles, so the loads of tile i+1 are in flight during the epilogue of tile i
-//   warpgroups 1, 2  wgmma m64nBNk16 on rows [0, 64) / [64, 128) of the tile (both operands from the 128B-swizzled ring),
-//                one k-block in flight behind the one being issued; then the epilogue of their 64 rows
+//                ring in one in-order sequence, without draining between tiles.  The warpgroup gives up registers
+//                (setmaxnreg) to the two MMA warpgroups.
+//   warpgroups 1, 2  own alternate tiles of the CTA's sequence (tiles 0, 2, 4, ... / 1, 3, 5, ...).  A warpgroup computes its
+//                whole 128 x BN tile as two wgmma m64nBNk16 row halves (both operands from the 128B-swizzled ring, one k-block
+//                in flight behind the one being issued), consumes only its own tiles' ring stages, and steps its ring
+//                position past the other warpgroup's.  Then it runs the epilogue of its tile while the other warpgroup's
+//                MMAs keep the tensor cores busy.
+//   The mainloops alternate strictly (an ordering barrier between the two MMA warpgroups): a warpgroup starts waiting on its
+//   next tile's stages only once the other one has seen all of its own.  Besides keeping the two mainloops from sharing the
+//   tensor cores, this keeps every full-barrier wait within one phase of the barrier, which the parity waits require.
 // Tiles are ordered n-fastest so CTAs that run concurrently share A tiles in L2.
 #include "gemm_common.cuh"
 #include "kernels.h"
@@ -32,9 +39,9 @@ struct GemmCfg {
   static_assert(B_BYTES % 1024 == 0, "stages must stay 1024-byte aligned (128B swizzle atoms)");
 };
 
-// Drain the accumulator fragments of one MMA warpgroup (64 rows x NCOLS columns) through the transpose buffer, 64 columns at
-// a time, and run the per-chunk epilogue with one row per thread: warp wl of the warpgroup takes rows (wl & 1) * 32 + lane
-// and chunk (wl >> 1) of each 64-column slab.
+// Drain the accumulator fragments of one 64-row half of an MMA warpgroup's tile (64 rows x NCOLS columns) through the
+// warpgroup's transpose buffer, 64 columns at a time, and run the per-chunk epilogue with one row per thread: warp wl of the
+// warpgroup takes rows (wl & 1) * 32 + lane of the half and chunk (wl >> 1) of each 64-column slab.
 template <int BN, int NCOLS>
 __device__ __forceinline__ void epi_drain(const GemmParams& p, const EpiTile& t, float (&acc)[BN / 2], float* xpose, int cw, int wl, int lane,
                                           uint8_t* stage, bool plain, int nb0, int col0, int n_out) {
@@ -88,14 +95,16 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tap_kernel(const __grid_
     if (p.out_tma) tma_prefetch_desc(&p.tmap_out);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], EPI_WARPS);          // one arrival per MMA warp
+      mbar_init(&empty_bar[s], 4);                  // one arrival per warp of the MMA warpgroup that owns the stage's tile
     }
     fence_barrier_init();
   }
   __syncthreads();
 
   // ring positions are carried as (index, phase bit) pairs and tile coordinates come from multiply-high divisions
-  if (warp == 0) {
+  if (warp < 4) {
+    setmaxnreg_dec<GEMM_PRODUCER_REGS>();
+    if (warp != 0) return;
     // ------------------------------ TMA producer ------------------------------
     // warp-uniform loop, ONE elected lane issues (keeps barrier / descriptor operands in uniform registers)
     int s = 0;
@@ -125,28 +134,43 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tap_kernel(const __grid_
         }
       }
     }
-  } else if (warp >= 4) {
+  } else {
     // ------------------------------ MMA warpgroups + epilogue ------------------------------
-    const int cw = (warp >> 2) - 1;                 // rows [64 cw, 64 cw + 64) of every tile
+    setmaxnreg_inc<GEMM_MMA_REGS>();
+    const int cw = (warp >> 2) - 1;                 // tiles cw, cw + 2, cw + 4, ... of this CTA's sequence
     const int wl = warp & 3;
     uint8_t* stage = epi_smem + (warp - 4) * EPI_STAGE_BYTES;
     float* xpose = reinterpret_cast<float*>(epi_smem + EPI_WARPS * EPI_STAGE_BYTES + cw * EPI_XPOSE_BYTES);
     const uint32_t ring = smem_u32(smem);
-    float acc[BN / 2];
+    float acc[2][BN / 2];                           // rows [0, 64) and [64, 128) of the tile
 #pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0.f;
     int s = 0;
     uint32_t ph = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    // step the ring position past the `iters` stages of a tile the other warpgroup consumes
+    auto skip_tile = [&]() {
+      s += iters;
+      ph ^= (uint32_t)(s / STAGES) & 1u;
+      s %= STAGES;
+    };
+    if (cw == 1) skip_tile();
+    for (int tile = blockIdx.x + cw * gridDim.x; tile < p.total_tiles; tile += 2 * gridDim.x) {
+      // ordering barrier: the other warpgroup has waited on every stage of the tile before this one (ids 3 / 4: "cw may start")
+      if (tile >= (int)gridDim.x) named_bar_sync(3 + cw, 256);
       int prev = -1;
       for (int i = 0; i < iters; ++i) {
         mbar_wait(&full_bar[s], ph);
-        const uint32_t a_addr = ring + s * Cfg::STAGE_BYTES + cw * (64 * BK * 2);
+        const uint32_t a_addr = ring + s * Cfg::STAGE_BYTES;
         const uint32_t b_addr = ring + s * Cfg::STAGE_BYTES + Cfg::A_BYTES;
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k)
-          Wgmma<BN>::ss(acc, wgmma_desc_sw128(a_addr + 32 * k), wgmma_desc_sw128(b_addr + 32 * k), (i > 0 || k > 0) ? 1 : 0);
+        for (int k = 0; k < BK / 16; ++k) {
+          const uint64_t db = wgmma_desc_sw128(b_addr + 32 * k);
+          Wgmma<BN>::ss(acc[0], wgmma_desc_sw128(a_addr + 32 * k), db, (i > 0 || k > 0) ? 1 : 0);
+          Wgmma<BN>::ss(acc[1], wgmma_desc_sw128(a_addr + 64 * BK * 2 + 32 * k), db, (i > 0 || k > 0) ? 1 : 0);
+        }
         wgmma_commit();
         wgmma_wait<1>();                            // the previous k-block's MMAs have retired: its stage may be refilled
         if (prev >= 0) {
@@ -156,47 +180,53 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tap_kernel(const __grid_
         prev = s;
         if (++s == STAGES) { s = 0; ph ^= 1; }
       }
+      if (tile + (int)gridDim.x < p.total_tiles) named_bar_arrive(4 - cw, 256);   // the other warpgroup's next tile may start
+      skip_tile();
       wgmma_wait<0>();
-      wgmma_fence_regs(acc);
+      wgmma_fence_regs(acc[0]);
+      wgmma_fence_regs(acc[1]);
       if (prev >= 0) {
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty_bar[prev]);
       }
-      const EpiTile t = epi_tile(p, tile, cw * 2 + (wl & 1), lane);
-      const int n0 = t.n_tile * BN;
-      if (!p.geglu) {
-        epi_drain<BN, BN>(p, t, acc, xpose, cw, wl, lane, stage, false, n0, n0, p.N);
-      } else {
-        // GEGLU on the fragments: tile columns [0, BN/2) are values, [BN/2, BN) the matching gates (weights were interleaved
-        // per tile); out[:, n_tile*BN/2 + c] = (value + bias_v) * gelu(gate + bias_g).  No residual (checked on the host).
-        constexpr int HALF = BN / 2;
-        const TileCoord tc = tile_coord_m(p, t.m_tile);
-        float2 ln[2] = {make_float2(0.f, 1.f), make_float2(0.f, 1.f)};
-        if (p.ln_stats) {
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int R = cw * 64 + 16 * wl + (lane >> 2) + 8 * h;
-            const int x = tc.x0 + (R & (p.bx - 1)), y = tc.y0 + (R >> p.bx_shift);
-            if (x < p.X && y < p.Y && tc.z < p.Z)
-              ln[h] = __ldg(reinterpret_cast<const float2*>(p.ln_stats) + ((long long)tc.z * p.Y + y) * p.X + x);
-          }
-        }
+      for (int h = 0; h < 2; ++h) {
+        const EpiTile t = epi_tile(p, tile, h * 2 + (wl & 1), lane);
+        const int n0 = t.n_tile * BN;
+        if (BN != 128 || !p.geglu) {                   // GEGLU always runs at BN = 128 (pick_bn)
+          epi_drain<BN, BN>(p, t, acc[h], xpose, cw, wl, lane, stage, false, n0, n0, p.N);
+        } else {
+          // GEGLU on the fragments: tile columns [0, BN/2) are values, [BN/2, BN) the matching gates (weights were interleaved
+          // per tile); out[:, n_tile*BN/2 + c] = (value + bias_v) * gelu(gate + bias_g).  No residual (checked on the host).
+          constexpr int HALF = BN / 2;
+          const TileCoord tc = tile_coord_m(p, t.m_tile);
+          float2 ln[2] = {make_float2(0.f, 1.f), make_float2(0.f, 1.f)};
+          if (p.ln_stats) {
 #pragma unroll
-        for (int j = 0; j < HALF / 8; ++j) {
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const int n = n0 + 8 * j + 2 * (lane & 3) + (e & 1);
-            float a = acc[j * 4 + e], g = acc[(j + HALF / 8) * 4 + e];
-            if (p.ln_stats) {
-              const float2 l = ln[e >> 1];
-              a = (a - l.x * __ldg(p.ln_colsum + n)) * l.y;
-              g = (g - l.x * __ldg(p.ln_colsum + n + HALF)) * l.y;
+            for (int r = 0; r < 2; ++r) {
+              const int R = h * 64 + 16 * wl + (lane >> 2) + 8 * r;
+              const int x = tc.x0 + (R & (p.bx - 1)), y = tc.y0 + (R >> p.bx_shift);
+              if (x < p.X && y < p.Y && tc.z < p.Z)
+                ln[r] = __ldg(reinterpret_cast<const float2*>(p.ln_stats) + ((long long)tc.z * p.Y + y) * p.X + x);
             }
-            if (t.bias) { a += __ldg(t.bias + n); g += __ldg(t.bias + n + HALF); }
-            acc[j * 4 + e] = a * gelu_epilogue(g);
           }
+#pragma unroll
+          for (int j = 0; j < HALF / 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const int n = n0 + 8 * j + 2 * (lane & 3) + (e & 1);
+              float a = acc[h][j * 4 + e], g = acc[h][(j + HALF / 8) * 4 + e];
+              if (p.ln_stats) {
+                const float2 l = ln[e >> 1];
+                a = (a - l.x * __ldg(p.ln_colsum + n)) * l.y;
+                g = (g - l.x * __ldg(p.ln_colsum + n + HALF)) * l.y;
+              }
+              if (t.bias) { a += __ldg(t.bias + n); g += __ldg(t.bias + n + HALF); }
+              acc[h][j * 4 + e] = a * gelu_epilogue(g);
+            }
+          }
+          epi_drain<BN, HALF>(p, t, acc[h], xpose, cw, wl, lane, stage, true, n0, t.n_tile * HALF, p.N / 2);
         }
-        epi_drain<BN, HALF>(p, t, acc, xpose, cw, wl, lane, stage, true, n0, t.n_tile * HALF, p.N / 2);
       }
     }
     if (p.out_tma && lane == 0) tma_store_wait_all();   // bulk stores must be complete before the CTA exits
