@@ -25,6 +25,8 @@
 namespace vc {
 
 static constexpr int PEER_MAX = 8;
+static constexpr int PEER_BMAX = 4;     // batch samples per collective (three-way guidance runs B=3 frame-sharded forwards)
+static constexpr int PEER_ALLREDUCE_THREADS = PEER_BMAX * 64;
 
 struct PeerCommDev {
   int world, rank;
@@ -61,6 +63,7 @@ __device__ __forceinline__ unsigned int ld_acquire_sys(const unsigned int* p) {
 
 // Tail of every collective, executed by ALL threads of the LAST CTA of this rank (the caller has established that every other
 // CTA's stores are fenced): publish `mine` (B*64 partial sums, or nothing), signal, wait for all peers, gather their sums.
+// Thread tid publishes sum tid, so the CTA must have at least B*64 threads (PEER_BMAX * 64 = 256).
 __device__ __forceinline__ void peer_finish(const PeerCommDev& pc, int B, bool with_stats, float mine, int tid) {
   const unsigned int s = *reinterpret_cast<volatile unsigned int*>(pc.seq) + 1u;
   const int n = B * 64;
@@ -191,7 +194,7 @@ __global__ void __launch_bounds__(512) peer_exchange_kernel(const __grid_constan
 // (sum, sumsq) per group of this rank's rows -> every rank's slots -> cur_stats[B][world][64]
 // B == 0: the signal / wait step alone -- the completion barrier of a layout switch that a GEMM's epilogue performed (its TMA stores to
 // the peers are complete when that kernel ends; this kernel, next in the stream, fences and publishes the sequence number).
-__global__ void __launch_bounds__(128) gn_peer_allreduce_kernel(const float* __restrict__ partial, int splits, int B, const __grid_constant__ PeerCommDev pc) {
+__global__ void __launch_bounds__(PEER_ALLREDUCE_THREADS) gn_peer_allreduce_kernel(const float* __restrict__ partial, int splits, int B, const __grid_constant__ PeerCommDev pc) {
   const int tid = threadIdx.x;
   float mine = 0.f;
   if (tid < B * 64) {
@@ -212,7 +215,8 @@ int groupnorm_stats_partials(const __half* x1, int C1, int samples, long long ro
 
 static int to_dev(const vc_peer_comm* c, PeerCommDev& d) {
   VC_REQUIRE(c && c->world >= 1 && c->world <= PEER_MAX && c->rank >= 0 && c->rank < c->world, "peer comm: bad world / rank");
-  VC_REQUIRE(c->flags && c->seq && c->done && c->cur_stats && c->Bmax >= 1 && c->Bmax <= 2, "peer comm: null buffer or Bmax not in 1..2");
+  VC_REQUIRE(c->flags && c->seq && c->done && c->cur_stats && c->Bmax >= 1 && c->Bmax <= PEER_BMAX, "peer comm: null buffer or Bmax not in 1..%d",
+             PEER_BMAX);
   d.world = c->world; d.rank = c->rank;
   d.flags = reinterpret_cast<unsigned int*>(c->flags);
   d.seq = reinterpret_cast<unsigned int*>(c->seq);
@@ -308,6 +312,7 @@ int vc_peer_exchange(const vc_peer_comm* c, const void* src, void* const* dst, i
   p.rows_per_split = (p.rows_local + splits - 1) / splits;
   p.partial = reinterpret_cast<float*>(ws);
   VC_REQUIRE(!p.with_stats || (ws && ws_bytes >= (size_t)B * splits * 64 * sizeof(float)), "peer_exchange: workspace too small");
+  VC_REQUIRE(p.vecs * p.ppi >= B * 64, "peer_exchange: %d threads cannot publish %d samples' statistics", p.vecs * p.ppi, B);
   dim3 grid(splits, B);
   peer_exchange_kernel<<<grid, p.vecs * p.ppi, p.with_stats ? (size_t)2 * C * p.ppi * sizeof(float) : 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
   VC_CHECK_CUDA(cudaGetLastError());
@@ -325,7 +330,7 @@ int vc_peer_groupnorm_stats(const vc_peer_comm* c, const void* x, int32_t C, int
   rc = groupnorm_stats_partials(reinterpret_cast<const __half*>(x), C, samples, rows_per_sample, reinterpret_cast<float*>(ws), ws_bytes,
                                 &splits, reinterpret_cast<cudaStream_t>(stream));
   if (rc) return rc;
-  gn_peer_allreduce_kernel<<<1, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(reinterpret_cast<const float*>(ws), splits, samples, d);
+  gn_peer_allreduce_kernel<<<1, PEER_ALLREDUCE_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(reinterpret_cast<const float*>(ws), splits, samples, d);
   VC_CHECK_CUDA(cudaGetLastError());
   return VC_OK;
 }
@@ -349,7 +354,7 @@ int vc_peer_finish_scatter(const vc_peer_comm* c, const vc_gn_part_geom* geom, i
     if (rc) return rc;
     B = samples;
   }
-  gn_peer_allreduce_kernel<<<1, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(reinterpret_cast<const float*>(ws), splits, B, d);
+  gn_peer_allreduce_kernel<<<1, PEER_ALLREDUCE_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(reinterpret_cast<const float*>(ws), splits, B, d);
   VC_CHECK_CUDA(cudaGetLastError());
   return VC_OK;
 }

@@ -4,7 +4,8 @@ Same constructor, ``make_schedule`` / ``sample`` / ``ddim_sampling`` / ``p_sampl
 (``(samples, {'x_inter': [...], 'pred_x0': [...]})``).  Host logic (schedule tables, loop, RNG draws with the same
 shapes in the same order) is Python; everything after the two ``apply_model`` calls of a step -- CFG combine,
 guidance rescale (two global unbiased stds), v->(eps, x0), dynamic rescale, x_{t-1} -- is ONE fused CUDA update
-(vc_ddim_update).  ``batch_cfg=True`` runs cond+uncond as a single B=2 U-Net forward.
+(vc_ddim_update).  ``batch_cfg=True`` runs cond+uncond as a single B=2 U-Net forward (the three-way sampler: cond, uncond
+and uncond_img as one B=3 forward).
 """
 from __future__ import annotations
 
@@ -139,22 +140,41 @@ class DDIMSampler(object):
                 intermediates['pred_x0'].append(pred_x0)
         return img, intermediates
 
-    def _stacked_conditioning(self, c, uc):
-        """cond|uncond conditioning stacked along the batch axis, built once per (c, uc) pair and reused for every step:
-        the sampler passes the same dicts for all steps (ddim.py:150-160), and handing the U-Net the SAME context tensor
-        each step lets it keep the cross-attention K/V projections (SURVEY.md App. C.1).  Also reports whether the
-        c_concat entries of the two branches are the same tensors (utils/diffusion_utils.py:152-153)."""
-        ents = [(a, u) for k in c for a, u in zip(c[k], uc[k])]
-        sig = [(a, ops.tensor_version(a), u, ops.tensor_version(u)) for a, u in ents]
+    def _stacked_conditioning(self, *conds):
+        """The conditionings of the guidance branches (cond | uncond [| uncond_img]) stacked along the batch axis, built once
+        per tuple of dicts and reused for every step: the sampler passes the same dicts for all steps (ddim.py:150-160), and
+        handing the U-Net the SAME context tensor each step lets it keep the cross-attention K/V projections (SURVEY.md
+        App. C.1).  Also reports whether the c_concat entries of all branches are the same tensors
+        (utils/diffusion_utils.py:152-153)."""
+        c0 = conds[0]
+        groups = [ents for k in c0 for ents in zip(*(c[k] for c in conds))]
+        sig = [(a, ops.tensor_version(a)) for ents in groups for a in ents]
         cached = getattr(self, "_cat_cache", None)
-        if cached is not None and len(cached[0]) == len(sig) and all(va is not None and vu is not None for _, va, _, vu in sig) and all(
-                a is a0 and va == va0 and u is u0 and vu == vu0 for (a, va, u, vu), (a0, va0, u0, vu0) in zip(sig, cached[0])):
-            return cached[1], cached[2]
-        cat = {k: [torch.cat([a, u], 0) for a, u in zip(c[k], uc[k])] for k in c}
-        same = all((a is u) or (a.shape == u.shape and bool(torch.equal(a, u))) for a, u in zip(c.get("c_concat", []), uc.get("c_concat", []))) \
-            if "c_concat" in c else False
-        self._cat_cache = (sig, cat, same)
+        if cached is not None and cached[0] == len(conds) and len(cached[1]) == len(sig) and all(v is not None for _, v in sig) and all(
+                a is a0 and v == v0 for (a, v), (a0, v0) in zip(sig, cached[1])):
+            return cached[2], cached[3]
+        cat = {k: [torch.cat(list(ents), 0) for ents in zip(*(c[k] for c in conds))] for k in c0}
+        same = "c_concat" in c0 and all((a is u) or (a.shape == u.shape and bool(torch.equal(a, u)))
+                                        for ents in zip(*(c["c_concat"] for c in conds)) for a, u in zip(ents, ents[1:]))
+        self._cat_cache = (len(conds), sig, cat, same)
         return cat, same
+
+    def _can_stack(self, *conds):
+        return self.batch_cfg and all(isinstance(c, dict) and c.keys() == conds[0].keys() for c in conds)
+
+    def _apply_stacked(self, x, t, conds, kwargs):
+        """The guidance branches `conds` as ONE U-Net forward of batch len(conds) * B; returns the per-branch predictions."""
+        n = len(conds)
+        cat, same_concat = self._stacked_conditioning(*conds)
+        kw = {k: (torch.cat([v] * n, 0) if isinstance(v, torch.Tensor) and v.dim() >= 1 and v.shape[0] == x.shape[0] else v)
+              for k, v in kwargs.items()}
+        if same_concat and x.shape[0] == 1:
+            # every branch sees the same x, t, fs and c_concat: let the U-Net compute the context-free prefix once
+            # (SURVEY.md App. C.2; ignored by models that do not know the hint)
+            kw["cfg_shared_prefix"] = True
+        out = self.model.apply_model(torch.cat([x] * n, 0), torch.cat([t] * n, 0), cat, **kw)
+        b = x.shape[0]
+        return [out[i * b:(i + 1) * b].contiguous() for i in range(n)]
 
     def _apply_both(self, x, t, c, uc, kwargs):
         """cond + uncond as one B=2 forward when every conditioning entry can be stacked; else two calls (ddim.py:223-224)."""
@@ -162,17 +182,8 @@ class DDIMSampler(object):
         if cfg is not None:                                   # multi-GPU CFG split: this rank computes one branch only
             mine = self.model.apply_model(x, t, c if cfg.branch == 0 else uc, **kwargs)
             return cfg.exchange(mine.float().contiguous())
-        if self.batch_cfg and isinstance(c, dict) and isinstance(uc, dict) and c.keys() == uc.keys():
-            cat, same_concat = self._stacked_conditioning(c, uc)
-            kw = {k: (torch.cat([v, v], 0) if isinstance(v, torch.Tensor) and v.dim() >= 1 and v.shape[0] == x.shape[0] else v)
-                  for k, v in kwargs.items()}
-            if same_concat and x.shape[0] == 1:
-                # both branches see the same x, t, fs and c_concat: let the U-Net compute the context-free prefix once
-                # (SURVEY.md App. C.2; ignored by models that do not know the hint)
-                kw["cfg_shared_prefix"] = True
-            out = self.model.apply_model(torch.cat([x, x], 0), torch.cat([t, t], 0), cat, **kw)
-            n = x.shape[0]
-            return out[:n].contiguous(), out[n:].contiguous()
+        if self._can_stack(c, uc):
+            return tuple(self._apply_stacked(x, t, (c, uc), kwargs))
         return self.model.apply_model(x, t, c, **kwargs), self.model.apply_model(x, t, uc, **kwargs)
 
     @torch.no_grad()

@@ -146,9 +146,11 @@ class PeerFrameComm(FrameComm):
       * the statistics of the 5-D GroupNorm that follows every to_sites ride along with it (no statistics pass, no all-reduce),
       * the GroupNorms in the middle of a temporal block exchange 2 x 32 floats per sample through the same flag protocol.
     The receive buffers are reused by every switch (one per direction): tensors returned by to_sites()/to_frames() are views
-    of them and are only valid until the next switch in the same direction -- UNetModel clones the ones it keeps as skips."""
+    of them and are only valid until the next switch in the same direction -- UNetModel clones the ones it keeps as skips.
+    Batches of up to `bmax` samples (4: the B=3 forward of three-way guidance); the receive buffers grow with the first
+    switch that needs more room."""
 
-    def __init__(self, dist, rank: int, world: int, group, device, bmax: int = 2):
+    def __init__(self, dist, rank: int, world: int, group, device, bmax: int = 4):
         super().__init__(dist, rank, world, group)
         from . import _lib
         self.lib = _lib.load()
@@ -360,15 +362,23 @@ class _ScatterPlan:
 class CfgComm:
     """Classifier-free-guidance split: the conditional and unconditional U-Net forwards of a DDIM step are independent
     (ddim.py:223-224), so the first half of the ranks computes `cond`, the second half `uncond`, and rank i swaps its
-    3.7 MB prediction with rank i + world/2 through a 2-rank all-gather."""
+    3.7 MB prediction with rank i + world/2 through a 2-rank all-gather.  Three-way guidance (ddim_multiplecond.py) puts
+    `uncond` and `uncond_img` on the second half, which then sends twice the rows of the first."""
 
     def __init__(self, dist, branch: int, pair_group):
         self.dist, self.branch, self.pair_group = dist, branch, pair_group
 
-    def exchange(self, v_mine: torch.Tensor):
-        buf = v_mine.new_empty((2, *v_mine.shape))
-        self.dist.all_gather_into_tensor(buf.view(-1), v_mine.contiguous().view(-1), group=self.pair_group)   # pair group rank order = (cond, uncond)
-        return buf[0], buf[1]
+    def exchange(self, v_mine: torch.Tensor, rows=None):
+        """-> (branch 0's prediction, branch 1's prediction).  `rows`: the batch rows of the two when they differ; the smaller
+        part is zero-padded to the larger for the all-gather."""
+        rows = rows or (v_mine.shape[0], v_mine.shape[0])
+        n = max(rows)
+        mine = v_mine.contiguous()
+        if mine.shape[0] < n:
+            mine = torch.cat([mine, mine.new_zeros((n - mine.shape[0], *mine.shape[1:]))], 0)
+        buf = v_mine.new_empty((2, n, *v_mine.shape[1:]))
+        self.dist.all_gather_into_tensor(buf.view(-1), mine.view(-1), group=self.pair_group)   # pair group rank order = (branch 0, branch 1)
+        return buf[0, :rows[0]], buf[1, :rows[1]]
 
 
 def _make_comm(dist, rank, world, group, device, peer: bool):

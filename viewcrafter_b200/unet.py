@@ -397,9 +397,9 @@ class UNetModel(nn.Module):
 
     @staticmethod
     def _spatial_tf(P, h, ctx, B, T, H, W, expand=False, out_plan=None):
-        """expand=True (shared CFG prefix, SURVEY.md App. C.2): `h` holds ONE batch element that is identical for the B=2
-        conditional / unconditional branches; everything up to and including attn1 of the first block does not see the
-        context, so it runs once and is duplicated right before the first cross-attention."""
+        """expand=True (shared CFG prefix, SURVEY.md App. C.2): `h` holds ONE batch element that is identical for all B
+        guidance branches (cond / uncond [/ uncond_img]); everything up to and including attn1 of the first block does not
+        see the context, so it runs once and is copied B times right before the first cross-attention."""
         Bc = 1 if expand else B
         BT, HW, heads = Bc * T, H * W, P["heads"]
         C = heads * 64
@@ -412,8 +412,8 @@ class UNetModel(nn.Module):
             x = ops.linear(a, Q["o1_w"], bias=Q["o1_b"], res=x, ln_out=fold)
             x, st = x if fold else (x, None)
             if expand:
-                x, h = torch.cat([x, x], 0), torch.cat([h, h], 0)
-                st = torch.cat([st, st], 0) if st is not None else None
+                x, h = torch.cat([x] * B, 0), torch.cat([h] * B, 0)
+                st = torch.cat([st] * B, 0) if st is not None else None
                 expand, Bc, BT = False, B, B * T
             q = _ln_linear(Q, x, "q2", "ln2", st)
             a = torch.empty_like(q)
@@ -601,10 +601,10 @@ class UNetModel(nn.Module):
         B, Cin, T, H, W = x.shape
         dev = x.device
         x32 = x.float().contiguous()
-        # cfg_shared_prefix: the caller (DDIMSampler._apply_both) asserts that batch rows 0 and 1 carry the same x, t, fs
+        # cfg_shared_prefix: the caller (DDIMSampler._apply_stacked) asserts that all B batch rows carry the same x, t, fs
         # and c_concat and differ only in the cross-attention context
         kinds = [Pm["kind"] for Pm in P["input"][1]] if len(P["input"]) > 1 else []
-        shared = bool(kwargs.get("cfg_shared_prefix")) and B == 2 and comm is None and kinds[:2] == ["R", "S"]
+        shared = bool(kwargs.get("cfg_shared_prefix")) and B >= 2 and comm is None and kinds[:2] == ["R", "S"]
         # --- embeddings (fp32) : time_embed(t) + fps_embedding(fs), one row per batch element (frame-invariant) ---
         ts = timesteps.to(device=dev, dtype=torch.int64).contiguous()
         tw = P["time"]
@@ -631,15 +631,15 @@ class UNetModel(nn.Module):
         hs = []
         first = 0
         if shared:
-            # SURVEY.md App. C.2: both CFG branches see the same x, t, fs and c_concat, so everything before the first
+            # SURVEY.md App. C.2: all CFG branches see the same x, t, fs and c_concat, so everything before the first
             # cross-attention (input_blocks.0, init_attn, input_blocks.1.0 and input_blocks.1.1 up to attn1) is computed once
-            # on one batch element and duplicated; the results are those of the plain B=2 forward.
+            # on one batch element and copied B times; the results are those of the plain batch-B forward.
             emb1 = emb[:1].contiguous()
             h = h[:T * H * W]
             h, H, W = self._run_stage(P["input"][0], h, None, emb1, ctx, 1, T, H, W)
             if self.addition_attention:
                 h, H, W = self._run_stage(P["init_attn"], h, None, emb1, ctx, 1, T, H, W)
-            hs.append(torch.cat([h, h], 0))
+            hs.append(torch.cat([h] * B, 0))
             Bc = 1
             for Pm in P["input"][1]:
                 if Bc == 1 and Pm["kind"] == "R":
