@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define VC_B200_ABI_VERSION 6
+#define VC_B200_ABI_VERSION 7
 
 int vc_abi_version(void);
 const char* vc_last_error(void);
@@ -137,6 +137,17 @@ size_t vc_groupnorm_parts_ws_bytes(int32_t samples);
 int vc_groupnorm_from_parts(const void* x1, int32_t C1, const vc_gn_part_geom* g1, const void* x2, int32_t C2, const vc_gn_part_geom* g2,
                             int32_t samples, int64_t rows_per_sample, const float* gamma, const float* beta, float eps, int32_t silu,
                             void* out, void* ws, size_t ws_bytes, void* stream);
+/* Reproducible mode: GroupNorm statistics from canonical "leaves" whose values and combine order do not depend on the batch, the
+ * frame sharding across GPUs or the SM count.  A leaf is the per-group (sum, sumsq) over one chunk of a frame: rows_per_leaf
+ * contiguous rows (H*W / nc pixels).  vc_groupnorm_leaves writes leaves[n_leaves][32][2] for the row blocks
+ * [n * rows_per_leaf, (n + 1) * rows_per_leaf) of concat(x1, x2).  vc_groupnorm_apply_leaves sums the leaves_per_sample consecutive
+ * leaves of each sample in index order (fp64) and normalises its rows_per_sample rows with the row count stat_rows
+ * (>= rows_per_sample: the site-sharded 5-D GroupNorm).  ws: >= samples * 64 floats. */
+int vc_groupnorm_leaves(const void* x1, int32_t C1, const void* x2, int32_t C2, int64_t n_leaves, int64_t rows_per_leaf, float* leaves,
+                        void* stream);
+int vc_groupnorm_apply_leaves(const void* x1, int32_t C1, const void* x2, int32_t C2, int32_t samples, int64_t rows_per_sample,
+                              const float* leaves, int32_t leaves_per_sample, int64_t stat_rows, const float* gamma, const float* beta,
+                              float eps, int32_t silu, void* out, void* ws, size_t ws_bytes, void* stream);
 /* statistics half of nn.LayerNorm: stats[row] = (mean, 1/sqrt(var + eps)) in fp32; the normalisation is applied by the
  * consuming vc_gemm_tap (ln_stats / ln_colsum), so the normalised activation is never written to memory */
 int vc_layernorm_stats(const void* x, int64_t rows, int32_t C, float eps, float* stats, void* stream);
@@ -178,6 +189,7 @@ typedef struct vc_ddim_scalars {
   float a_prev, sigma_t;
   float scale_t, prev_scale_t;
   int32_t use_cfg;
+  int32_t reproducible;              /* 1: a fixed statistics grid, independent of the SM count (reproducible mode) */
 } vc_ddim_scalars;
 int vc_ddim_update(const float* x, const float* v_cond, const float* v_uncond, const float* noise, float* x_prev, float* pred_x0,
                    int64_t n, const vc_ddim_scalars* s, void* ws /* 4 * 1025 doubles */, void* stream);
@@ -221,6 +233,12 @@ int vc_peer_exchange(const vc_peer_comm* c, const void* src, void* const* dst, i
 int vc_peer_finish_scatter(const vc_peer_comm* c, const vc_gn_part_geom* geom, int32_t C, int32_t samples, void* ws, size_t ws_bytes, void* stream);
 int vc_peer_groupnorm_stats(const vc_peer_comm* c, const void* x, int32_t C, int32_t samples, int64_t rows_per_sample, void* ws,
                             size_t ws_bytes, void* stream);
+/* Reproducible mode: the leaves of a site-layout 5-D GroupNorm.  leaves = this rank's [B][T][nc / world][64]; every rank's copy is
+ * stored into every rank's leaf buffer (dst[p]: rank p's float[2][cap] as mapped here, double-buffered by the collective's sequence
+ * number) at its canonical place [B][T][nc][64] (rank r holds chunks [r nc / world, (r + 1) nc / world)); after the rendezvous the
+ * full canonical array is copied to gathered[B][T][nc][64] for vc_groupnorm_apply_leaves. */
+int vc_peer_gather_leaves(const vc_peer_comm* c, const float* leaves, void* const* dst, int64_t cap, int32_t B, int32_t T, int32_t nc,
+                          float* gathered, void* stream);
 
 #ifdef __cplusplus
 }

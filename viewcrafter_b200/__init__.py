@@ -8,5 +8,9 @@ Drop-in classes (same names / constructor kwargs / state-dict keys as the refere
     viewcrafter_b200.resampler.Resampler        <- lvdm.modules.encoders.resampler.Resampler
     viewcrafter_b200.synthesis.image_guided_synthesis / get_latent_z <- utils.diffusion_utils (same names)
 All tensor work runs in libvc_b200.so (hand-written CUDA for sm_90a, C ABI in include/vc_b200.h).
+
+set_reproducible(on) / VC_REPRODUCIBLE=1: reproducible mode (bit-identical results across batching, GPU count and SM count).
 """
 __version__ = "0.1.0"
+
+from .ops import reproducible, set_reproducible  # noqa: E402,F401

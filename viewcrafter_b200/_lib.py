@@ -10,7 +10,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("VC_B200_LIB") or os.path.join(_HERE, "libvc_b200.so")   # override: A/B builds of the kernels
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 
 class VcError(RuntimeError):
@@ -49,7 +49,7 @@ class AttnDesc(C.Structure):
 class DdimScalars(C.Structure):
     _fields_ = [("cfg_scale", C.c_float), ("guidance_rescale", C.c_float), ("sqrt_ac_t", C.c_float),
                 ("sqrt_1mac_t", C.c_float), ("a_prev", C.c_float), ("sigma_t", C.c_float),
-                ("scale_t", C.c_float), ("prev_scale_t", C.c_float), ("use_cfg", C.c_int32)]
+                ("scale_t", C.c_float), ("prev_scale_t", C.c_float), ("use_cfg", C.c_int32), ("reproducible", C.c_int32)]
 
 
 class PeerComm(C.Structure):
@@ -87,6 +87,9 @@ SIGNATURES = {
                                    _vp, _sz, _vp]),
     "vc_peer_finish_scatter": (C.c_int, [C.POINTER(PeerComm), _vp, _i32, _i32, _vp, _sz, _vp]),
     "vc_peer_groupnorm_stats": (C.c_int, [C.POINTER(PeerComm), _vp, _i32, _i32, _i64, _vp, _sz, _vp]),
+    "vc_groupnorm_leaves": (C.c_int, [_vp, _i32, _vp, _i32, _i64, _i64, _vp, _vp]),
+    "vc_groupnorm_apply_leaves": (C.c_int, [_vp, _i32, _vp, _i32, _i32, _i64, _vp, _i32, _i64, _vp, _vp, _f32, _i32, _vp, _vp, _sz, _vp]),
+    "vc_peer_gather_leaves": (C.c_int, [C.POINTER(PeerComm), _vp, C.POINTER(C.c_void_p), _i64, _i32, _i32, _i32, _vp, _vp]),
     "vc_layernorm_stats": (C.c_int, [_vp, _i64, _i32, _f32, _vp, _vp]),
     "vc_layernorm_stats_from_parts": (C.c_int, [_vp, _i64, _i32, _f32, _vp, _vp]),
     "vc_layernorm": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _f32, _vp, _vp]),

@@ -103,6 +103,18 @@ int vc_groupnorm_apply_parts(const void* x1, int32_t C1, int32_t samples, int64_
   COUNT(1);
   return groupnorm_apply(H(x1), C1, nullptr, 0, samples, rows_per_sample, parts, stat_rows, gamma, beta, eps, silu, HM(out), ST(stream), n_parts);
 }
+int vc_groupnorm_leaves(const void* x1, int32_t C1, const void* x2, int32_t C2, int64_t n_leaves, int64_t rows_per_leaf, float* leaves,
+                        void* stream) {
+  COUNT(1);
+  return groupnorm_leaves(H(x1), C1, H(x2), C2, n_leaves, rows_per_leaf, leaves, ST(stream));
+}
+int vc_groupnorm_apply_leaves(const void* x1, int32_t C1, const void* x2, int32_t C2, int32_t samples, int64_t rows_per_sample,
+                              const float* leaves, int32_t leaves_per_sample, int64_t stat_rows, const float* gamma, const float* beta,
+                              float eps, int32_t silu, void* out, void* ws, size_t ws_bytes, void* stream) {
+  COUNT(2);
+  return groupnorm_apply_leaves(H(x1), C1, H(x2), C2, samples, rows_per_sample, leaves, leaves_per_sample, stat_rows, gamma, beta, eps, silu,
+                                HM(out), reinterpret_cast<float*>(ws), ws_bytes, ST(stream));
+}
 int vc_layernorm_stats(const void* x, int64_t rows, int32_t C, float eps, float* stats, void* stream) {
   COUNT(1);
   return layernorm_stats(H(x), rows, C, eps, stats, ST(stream));
@@ -173,6 +185,7 @@ int vc_ddim_update(const float* x, const float* v_cond, const float* v_uncond, c
   DdimStepScalars d;
   d.cfg_scale = s->cfg_scale; d.guidance_rescale = s->guidance_rescale; d.sqrt_ac_t = s->sqrt_ac_t; d.sqrt_1mac_t = s->sqrt_1mac_t;
   d.a_prev = s->a_prev; d.sigma_t = s->sigma_t; d.scale_t = s->scale_t; d.prev_scale_t = s->prev_scale_t; d.use_cfg = s->use_cfg;
+  d.reproducible = s->reproducible;
   COUNT((d.use_cfg && d.guidance_rescale > 0.f) ? 2 : 1);
   return ddim_update(x, v_cond, v_uncond, nullptr, 0.f, noise, x_prev, pred_x0, n, d, reinterpret_cast<double*>(ws), ST(stream));
 }
@@ -183,6 +196,7 @@ int vc_ddim_update3(const float* x, const float* v_cond, const float* v_uncond, 
   DdimStepScalars d;
   d.cfg_scale = s->cfg_scale; d.guidance_rescale = s->guidance_rescale; d.sqrt_ac_t = s->sqrt_ac_t; d.sqrt_1mac_t = s->sqrt_1mac_t;
   d.a_prev = s->a_prev; d.sigma_t = s->sigma_t; d.scale_t = s->scale_t; d.prev_scale_t = s->prev_scale_t; d.use_cfg = s->use_cfg;
+  d.reproducible = s->reproducible;
   COUNT((d.use_cfg && d.guidance_rescale > 0.f) ? 2 : 1);
   return ddim_update(x, v_cond, v_uncond, v_uncond_img, cfg_img, noise, x_prev, pred_x0, n, d, reinterpret_cast<double*>(ws), ST(stream));
 }

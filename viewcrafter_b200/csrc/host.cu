@@ -2,6 +2,7 @@
 #include <atomic>
 #include <cstdarg>
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 
 #include "common.cuh"
@@ -27,6 +28,10 @@ int sm_count() {
   int n = cache[slot].load(std::memory_order_relaxed);
   if (n == 0) {
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
+    // VC_SM_COUNT=k (k below the real count) sizes every launch grid as if the device had k SMs: it shows that the results of
+    // reproducible mode do not depend on the SM count (e.g. 114 of the PCIe H100 on a 132-SM card).  It can only shrink grids.
+    const char* e = getenv("VC_SM_COUNT");
+    if (e && atoi(e) > 0 && atoi(e) < n) n = atoi(e);
     cache[slot].store(n, std::memory_order_relaxed);
   }
   return n;

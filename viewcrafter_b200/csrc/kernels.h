@@ -76,6 +76,13 @@ int groupnorm_stats(const __half* x1, int C1, const __half* x2, int C2, int samp
 int groupnorm_apply(const __half* x1, int C1, const __half* x2, int C2, int samples, long long rows_per_sample,
                     const float* stats, long long stat_rows, const float* gamma, const float* beta, float eps, int silu, __half* out,
                     cudaStream_t stream, int stat_parts = 1);
+// Reproducible mode: leaves[n][32][2] = per-group (sum, sumsq) of the row blocks [n * rows_per_leaf, (n + 1) * rows_per_leaf), and the
+// normalise step whose statistics are the sums of leaves_per_sample consecutive leaves per sample, combined in index order.
+int groupnorm_leaves(const __half* x1, int C1, const __half* x2, int C2, long long n_leaves, long long rows_per_leaf, float* leaves,
+                     cudaStream_t stream);
+int groupnorm_apply_leaves(const __half* x1, int C1, const __half* x2, int C2, int samples, long long rows_per_sample, const float* leaves,
+                           int leaves_per_sample, long long stat_rows, const float* gamma, const float* beta, float eps, int silu,
+                           __half* out, float* ws, size_t ws_bytes, cudaStream_t stream);
 
 // GroupNorm(32) (+SiLU) whose statistics come from the gn_part records of the GEMM(s) that produced x1 (and x2): no statistics pass.
 struct GnPartGeom {
@@ -123,6 +130,7 @@ struct DdimStepScalars {
   float a_prev, sigma_t;            // ddim tables gathered by index
   float scale_t, prev_scale_t;      // dynamic rescale
   int use_cfg;
+  int reproducible = 0;             // 1: launch grid independent of the SM count
 };
 // v_uncond_img != nullptr: three-way CFG of ddim_multiplecond.py:227-233 with weight cfg_img on the image-only branch
 int ddim_update(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img, const float* noise,

@@ -225,6 +225,7 @@ __device__ __forceinline__ float cfg_combine(float c, float u, const float* __re
 // deterministic: every block leaves its four partial sums in ws[4 + 4 * block] (fixed in-block order); ddim_apply_kernel adds the
 // blocks up in index order -- no floating-point atomics, a seeded sampling run is bit-reproducible
 static constexpr int DDIM_MAX_BLOCKS = 1024;
+static constexpr int DDIM_REPRO_BLOCKS = 512;
 __global__ void __launch_bounds__(256) ddim_stats_kernel(const float* __restrict__ vc_, const float* __restrict__ vu, const float* __restrict__ vi, long long n,
                                   float cfg, float cfg_img, double* ws) {
   __shared__ double red[8][4];
@@ -291,7 +292,9 @@ int ddim_update(const float* x, const float* v_cond, const float* v_uncond, cons
   VC_REQUIRE(x && v_cond && noise && x_prev && pred_x0 && ws && n > 1, "ddim_update: bad args");
   VC_REQUIRE(!s.use_cfg || v_uncond, "ddim_update: CFG needs the unconditional output");
   VC_REQUIRE(!v_uncond_img || s.use_cfg, "ddim_update: the image-only branch is only defined with CFG on");
-  int blocks = (int)min((long long)sm_count() * 4, (n + 255) / 256);
+  // reproducible mode: a fixed number of statistics blocks, so the grid-strided order of the two std reductions does not depend on
+  // the SM count
+  int blocks = (int)min(s.reproducible ? (long long)DDIM_REPRO_BLOCKS : (long long)sm_count() * 4, (n + 255) / 256);
   if (blocks > DDIM_MAX_BLOCKS) blocks = DDIM_MAX_BLOCKS;
   if (s.use_cfg && s.guidance_rescale > 0.f) {           // ws: 4 * (1 + DDIM_MAX_BLOCKS) doubles
     ddim_stats_kernel<<<blocks, 256, 0, stream>>>(v_cond, v_uncond, v_uncond_img, n, s.cfg_scale, cfg_img, ws);

@@ -350,6 +350,57 @@ int groupnorm_apply(const __half* x1, int C1, const __half* x2, int C2, int samp
 }
 
 // ------------------------------------------------------------------------------------------------
+// Reproducible mode: canonical GroupNorm statistics ("leaves").  A leaf is the (sum, sumsq) per group of one block of
+// rows_per_leaf contiguous rows (one chunk of a frame's pixels); one CTA computes one leaf with the thread mapping and fixed
+// reduction order of gn_stats_dev, so a leaf depends only on its rows and on (rows_per_leaf, C1, C2) -- not on where the block
+// sits, how many leaves the launch has or the SM count.  The frame layout and the site layout of the multi-GPU U-Net hold the
+// same chunks whole, so both produce bit-identical leaves.
+__global__ void __launch_bounds__(512) gn_leaves_kernel(const __half* __restrict__ x1, const __half* __restrict__ x2, GnGeom g,
+                                                        float* __restrict__ leaves) {
+  gn_stats_dev(x1, x2, g, leaves, 0, blockIdx.x);
+}
+
+// stats[s][64] = sum of the leaves [s * per_sample, (s + 1) * per_sample) in index order (fp64, rounded once to fp32)
+__global__ void __launch_bounds__(64) gn_leaves_combine_kernel(const float* __restrict__ leaves, int per_sample, float* __restrict__ stats) {
+  const int s = blockIdx.x, t = threadIdx.x;
+  const float* p = leaves + (long long)s * per_sample * 64 + t;
+  double acc = 0.0;
+  int i = 0;
+  for (; i + 8 <= per_sample; i += 8) {            // loads first, then the adds in index order
+    float v[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) v[k] = __ldg(p + (long long)(i + k) * 64);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) acc += (double)v[k];
+  }
+  for (; i < per_sample; ++i) acc += (double)__ldg(p + (long long)i * 64);
+  stats[s * 64 + t] = (float)acc;
+}
+
+int groupnorm_leaves(const __half* x1, int C1, const __half* x2, int C2, long long n_leaves, long long rows_per_leaf, float* leaves,
+                     cudaStream_t stream) {
+  VC_REQUIRE(leaves && n_leaves >= 1 && n_leaves <= 0x7fffffffll, "groupnorm_leaves: bad args");
+  GnGeom g;
+  int rc = gn_geometry(g, x1, C1, x2, C2, 1, rows_per_leaf);
+  if (rc) return rc;
+  g.splits = 1; g.rows_per_split = rows_per_leaf;      // one CTA per leaf: nothing below depends on the device
+  g.stat_splits = 1; g.stat_rows = rows_per_leaf;
+  gn_leaves_kernel<<<(unsigned)n_leaves, g.vecs * g.ppi, (size_t)2 * g.C * g.ppi * sizeof(float), stream>>>(x1, x2, g, leaves);
+  VC_CHECK_CUDA(cudaGetLastError());
+  return VC_OK;
+}
+
+int groupnorm_apply_leaves(const __half* x1, int C1, const __half* x2, int C2, int samples, long long rows_per_sample, const float* leaves,
+                           int leaves_per_sample, long long stat_rows, const float* gamma, const float* beta, float eps, int silu,
+                           __half* out, float* ws, size_t ws_bytes, cudaStream_t stream) {
+  VC_REQUIRE(leaves && ws && samples >= 1 && leaves_per_sample >= 1, "groupnorm_apply_leaves: bad args");
+  VC_REQUIRE(ws_bytes >= (size_t)samples * 64 * sizeof(float), "groupnorm_apply_leaves: workspace too small");
+  gn_leaves_combine_kernel<<<samples, 64, 0, stream>>>(leaves, leaves_per_sample, ws);
+  VC_CHECK_CUDA(cudaGetLastError());
+  return groupnorm_apply(x1, C1, x2, C2, samples, rows_per_sample, ws, stat_rows, gamma, beta, eps, silu, out, stream, 1);
+}
+
+// ------------------------------------------------------------------------------------------------
 // GroupNorm from the partial sums the producing GEMM left behind (GemmDesc::gn_part, gemm_common.cuh: gn_part_accumulate):
 // the statistics pass over the activation disappears -- a small kernel folds the per-(32-row block, chunk, piece) records
 // (1.6 % of the activation's bytes) into per-(sample, split, group) sums in a fixed order, and gn_apply_kernel normalises in

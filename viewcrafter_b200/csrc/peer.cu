@@ -204,6 +204,35 @@ __global__ void __launch_bounds__(PEER_ALLREDUCE_THREADS) gn_peer_allreduce_kern
   peer_finish(pc, B, B > 0, mine, tid);
 }
 
+// Reproducible mode: gather the GroupNorm leaves of a site-layout tensor.  Rank r holds chunks [r ncl, (r + 1) ncl) of every frame and
+// stores its leaves straight into their canonical place of every rank's leaf buffer (half `parity` of [2][cap]: a rank can only be
+// writing collective s after every peer signalled s - 1, which in the peer's stream order follows the copy-out of collective s - 2).
+// After the rendezvous the full [B][T][nc][64] array is copied out of the own buffer: the leaves are exact copies, so every rank
+// (and a single GPU) combines the same values in the same order.
+struct LeafDst {
+  float* p[PEER_MAX];
+};
+__global__ void __launch_bounds__(512) peer_leaves_kernel(const float* __restrict__ leaves, const __grid_constant__ LeafDst dst, long long cap,
+                                                          int B, int T, int nc, float* __restrict__ gathered, const __grid_constant__ PeerCommDev pc) {
+  const int tid = threadIdx.x;
+  const unsigned int s = *reinterpret_cast<volatile unsigned int*>(pc.seq) + 1u;
+  const long long half = (long long)(s & 1u) * cap;
+  const int ncl = nc / pc.world;
+  const long long n4 = (long long)B * T * ncl * 16;                // float4s of this rank's leaves
+  for (long long i = tid; i < n4; i += blockDim.x) {
+    const long long leaf = i >> 4;
+    const long long bt = leaf / ncl, cl = leaf - bt * ncl;
+    const long long off = half + ((bt * nc + (long long)pc.rank * ncl + cl) * 64) + (i & 15) * 4;
+    const float4 v = __ldg(reinterpret_cast<const float4*>(leaves) + i);
+    for (int q = 0; q < pc.world; ++q) *reinterpret_cast<float4*>(dst.p[q] + off) = v;
+  }
+  peer_finish(pc, 0, false, 0.f, tid);
+  __threadfence_system();
+  const float4* own = reinterpret_cast<const float4*>(dst.p[pc.rank] + half);
+  const long long all4 = (long long)B * T * nc * 16;
+  for (long long i = tid; i < all4; i += blockDim.x) reinterpret_cast<float4*>(gathered)[i] = __ldcg(own + i);
+}
+
 }  // namespace vc
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -355,6 +384,25 @@ int vc_peer_finish_scatter(const vc_peer_comm* c, const vc_gn_part_geom* geom, i
     B = samples;
   }
   gn_peer_allreduce_kernel<<<1, PEER_ALLREDUCE_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(reinterpret_cast<const float*>(ws), splits, B, d);
+  VC_CHECK_CUDA(cudaGetLastError());
+  return VC_OK;
+}
+
+int vc_peer_gather_leaves(const vc_peer_comm* c, const float* leaves, void* const* dst, int64_t cap, int32_t B, int32_t T, int32_t nc,
+                          float* gathered, void* stream) {
+  using namespace vc;
+  PeerCommDev d;
+  int rc = to_dev(c, d);
+  if (rc) return rc;
+  VC_REQUIRE(leaves && dst && gathered && B >= 1 && T >= 1 && nc >= 1 && nc % c->world == 0, "peer_gather_leaves: bad args (nc %d, world %d)",
+             nc, c->world);
+  VC_REQUIRE((long long)B * T * nc * 64 <= cap, "peer_gather_leaves: %d x %d x %d leaves exceed the buffer", B, T, nc);
+  LeafDst ld;
+  for (int q = 0; q < c->world; ++q) {
+    VC_REQUIRE(dst[q], "peer_gather_leaves: null destination");
+    ld.p[q] = reinterpret_cast<float*>(dst[q]);
+  }
+  peer_leaves_kernel<<<1, 512, 0, reinterpret_cast<cudaStream_t>(stream)>>>(leaves, ld, cap, B, T, nc, gathered, d);
   VC_CHECK_CUDA(cudaGetLastError());
   return VC_OK;
 }

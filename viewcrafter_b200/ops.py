@@ -154,6 +154,36 @@ GN_FROM_PRODUCER = int(os.environ.get("VC_GN_FROM_PRODUCER", "1"))
 # over 50 frames, B = 2): producer sums 283 vs 364 us at 295 MB (level 0), 149 vs 194 at 147 MB, 92 vs 125 at 74 MB, 48 vs 53 at 18 MB
 # (level 3) -- the producer sums win at every U-Net level, so the threshold sits below the smallest one
 GN_PARTS_MIN_MB = float(os.environ.get("VC_GN_PARTS_MIN_MB", "16"))
+# Reproducible mode (set_reproducible / VC_REPRODUCIBLE=1): the same seed gives bit-identical results whatever the batching of the CFG
+# branches, the number of GPUs the frames are sharded over, per-frame or batched VAE calls and the SM count of the H100.  GroupNorm
+# statistics come from canonical leaves (groupnorm_canonical), the DDIM update launches a fixed grid.  Off by default: the default path
+# picks its GroupNorm splits and statistics source for speed, which changes the summation order with the layout.
+REPRODUCIBLE = os.environ.get("VC_REPRODUCIBLE", "0") == "1"
+
+
+def set_reproducible(on: bool = True) -> bool:
+    """Switch reproducible mode for the whole process; returns the previous setting.  Models that replay CUDA graphs recapture."""
+    global REPRODUCIBLE
+    prev, REPRODUCIBLE = REPRODUCIBLE, bool(on)
+    return prev
+
+
+def reproducible() -> bool:
+    return REPRODUCIBLE
+
+
+def gn_leaf_chunks(hw: int) -> int:
+    """nc: the chunks a frame of `hw` pixels is cut into for the canonical GroupNorm leaves.  A function of hw alone; a multiple of 8
+    whenever hw is (so that the site layout of 2, 4 or 8 GPUs holds whole chunks), doubled while a chunk keeps >= 256 pixels and up to
+    1024 chunks, so that even one frame of the VAE decoder (576x1024) spreads over the whole GPU.  1 if hw % 8 != 0."""
+    if hw % 8 != 0:
+        return 1
+    nc = 8
+    while nc < 1024 and hw % (2 * nc) == 0 and hw // (2 * nc) >= 256:
+        nc *= 2
+    return nc
+
+
 GN_SUB = 10          # sub-group width the U-Net producers cut their chunks at: every GroupNorm(32) boundary of 320 / 640 / 1280 channels
                      # and of their skip concats (640 / 960 / 1280 / 1920 / 2560) is a multiple of 10
 
@@ -198,7 +228,8 @@ def _gn_part_alloc(d: GemmDesc, device):
 
 
 def _want_gn(gn_out: bool, k_iters: int) -> bool:
-    return bool(gn_out) and (GN_FROM_PRODUCER >= 2 or (GN_FROM_PRODUCER == 1 and k_iters >= 12))
+    # reproducible mode never reads the producer's sums (their order follows the GEMM's tiling of the whole batch)
+    return bool(gn_out) and not REPRODUCIBLE and (GN_FROM_PRODUCER >= 2 or (GN_FROM_PRODUCER == 1 and k_iters >= 12))
 
 
 def gn_part_of(t):
@@ -271,7 +302,7 @@ def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None
 def _peer_gemm(d: GemmDesc, peer, device):
     """Launch a GEMM whose epilogue performs a multi-GPU layout switch (parallel._ScatterPlan) and complete the switch."""
     peer.attach(d)
-    part = _gn_part_alloc(d, device) if peer.to_sites else None      # frames -> sites: the cross-rank GroupNorm sums come from these records
+    part = _gn_part_alloc(d, device) if (peer.to_sites and not REPRODUCIBLE) else None      # frames -> sites: the cross-rank GroupNorm sums come from these records
     _gemm(d)
     return peer.finish(part)
 
@@ -462,7 +493,10 @@ def _gn_workspace(device, samples: int) -> torch.Tensor:
 def groupnorm(x: torch.Tensor, samples: int, gamma: torch.Tensor, beta: torch.Tensor, eps: float, silu: bool,
               x2: Optional[torch.Tensor] = None) -> torch.Tensor:
     """GroupNorm(32) (+SiLU) over ``samples`` groups of rows; [x|x2] concatenated along channels.  When the GEMMs that produced x
-    (and x2) left their partial sums (``_vc_gn``, see linear(gn_out=True)) the statistics pass is skipped: one read + one write."""
+    (and x2) left their partial sums (``_vc_gn``, see linear(gn_out=True)) the statistics pass is skipped: one read + one write.
+    Reproducible mode: a sample is one frame, its statistics come from canonical leaves (groupnorm_canonical)."""
+    if REPRODUCIBLE:
+        return groupnorm_canonical(x, samples, x.shape[0] // samples, gamma, beta, eps, silu, x2=x2)
     _chk16(x, "groupnorm.x")
     rows, C1 = x.shape
     C2 = 0 if x2 is None else x2.shape[1]
@@ -491,6 +525,45 @@ def groupnorm(x: torch.Tensor, samples: int, gamma: torch.Tensor, beta: torch.Te
     check(_lib.load().vc_groupnorm_nhwc(x.data_ptr(), C1, _ptr(x2), C2, samples, rows // samples, gamma.data_ptr(), beta.data_ptr(),
                                         eps, int(silu), out.data_ptr(), ws.data_ptr(), ws.numel(), _stream()), "vc_groupnorm_nhwc")
     return out
+
+
+def groupnorm_leaves(x: torch.Tensor, rows_per_leaf: int, x2: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """fp32 [rows / rows_per_leaf, 32, 2]: per-group (sum, sumsq) of every block of rows_per_leaf contiguous rows of [x|x2].  A leaf
+    depends only on its rows, rows_per_leaf and the channel counts (one CTA per leaf, fixed order)."""
+    _chk16(x, "groupnorm_leaves.x")
+    rows, C1 = x.shape
+    C2 = 0 if x2 is None else x2.shape[1]
+    assert x.is_contiguous() and (x2 is None or x2.is_contiguous()) and rows % rows_per_leaf == 0
+    leaves = torch.empty((rows // rows_per_leaf, 32, 2), device=x.device, dtype=torch.float32)
+    check(_lib.load().vc_groupnorm_leaves(x.data_ptr(), C1, _ptr(x2), C2, rows // rows_per_leaf, rows_per_leaf, leaves.data_ptr(), _stream()),
+          "vc_groupnorm_leaves")
+    return leaves
+
+
+def groupnorm_apply_leaves(x: torch.Tensor, samples: int, leaves: torch.Tensor, stat_rows: int, gamma: torch.Tensor, beta: torch.Tensor,
+                           eps: float, silu: bool, x2: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Normalise ``samples`` groups of rows of [x|x2] with statistics = the sum, in index order, of each sample's share of the leaves
+    ([samples * k, 32, 2], k consecutive leaves per sample) over ``stat_rows`` rows per sample."""
+    _chk16(x, "groupnorm_apply_leaves.x")
+    rows, C1 = x.shape
+    C2 = 0 if x2 is None else x2.shape[1]
+    assert leaves.dtype == torch.float32 and leaves.is_contiguous() and leaves.shape[0] % samples == 0
+    out = torch.empty((rows, C1 + C2), device=x.device, dtype=torch.float16)
+    ws = _gn_workspace(x.device, samples)
+    check(_lib.load().vc_groupnorm_apply_leaves(x.data_ptr(), C1, _ptr(x2), C2, samples, rows // samples, leaves.data_ptr(),
+                                                leaves.shape[0] // samples, stat_rows, gamma.data_ptr(), beta.data_ptr(), eps, int(silu),
+                                                out.data_ptr(), ws.data_ptr(), ws.numel(), _stream()), "vc_groupnorm_apply_leaves")
+    return out
+
+
+def groupnorm_canonical(x: torch.Tensor, samples: int, hw: int, gamma: torch.Tensor, beta: torch.Tensor, eps: float, silu: bool,
+                        x2: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """GroupNorm(32) (+SiLU) of ``samples`` groups of rows whose rows are (frame, pixel) with ``hw`` pixels per frame, from canonical
+    leaves: every frame is cut into gn_leaf_chunks(hw) chunks, a leaf is (frame, chunk, group), and a sample's statistics are its leaves
+    summed over frames, then chunks, in index order.  The result does not depend on how many samples the call holds, on the GPU
+    count the frames are sharded over or on the SM count (hw = rows per sample: a per-frame GroupNorm)."""
+    leaves = groupnorm_leaves(x, hw // gn_leaf_chunks(hw), x2=x2)
+    return groupnorm_apply_leaves(x, samples, leaves, x.shape[0] // samples, gamma, beta, eps, silu, x2=x2)
 
 
 def groupnorm_stats(x: torch.Tensor, samples: int) -> torch.Tensor:
@@ -641,6 +714,7 @@ def ddim_update(x, v_cond, v_uncond, noise, sc: dict, v_uncond_img=None, cfg_img
     s.sqrt_ac_t, s.sqrt_1mac_t = sc["sqrt_ac_t"], sc["sqrt_1mac_t"]
     s.a_prev, s.sigma_t, s.scale_t, s.prev_scale_t = sc["a_prev"], sc["sigma_t"], sc["scale_t"], sc["prev_scale_t"]
     s.use_cfg = int(use_cfg)
+    s.reproducible = int(REPRODUCIBLE)
     key = (x.device, torch.cuda.current_stream().cuda_stream)
     ws = _ddim_ws.get(key)
     if ws is None:

@@ -120,11 +120,41 @@ class FrameComm:
         """GroupNorm(32) of a site-layout tensor whose statistics span the ranks of the group.  `fresh`: x is the tensor the
         last to_sites() returned (the peer-memory path already holds its statistics)."""
         from . import ops
+        if ops.reproducible():
+            return self._groupnorm5d_leaves(x, B, gamma, beta, eps, silu, stat_rows)
         st = ops.groupnorm_stats(x, B)
         e0 = self._mark()
         self.all_reduce(st)
         self._done(e0)
         return ops.groupnorm_apply(x, B, st, stat_rows, gamma, beta, eps, silu)
+
+    # -- reproducible mode: canonical GroupNorm leaves (ops.groupnorm_canonical) ------------------------------------------------
+    def leaf_geometry(self, stat_rows: int):
+        """(HW, nc, rows per leaf) of a site-layout 5-D GroupNorm over stat_rows = T * HW rows per sample: this rank holds the chunks
+        [rank * nc / P, (rank + 1) * nc / P) of every frame, whole, so its leaves are exactly those of a single GPU."""
+        from . import ops
+        HW = stat_rows // self.T
+        nc = ops.gn_leaf_chunks(HW)
+        if nc % self.world != 0:
+            raise ValueError(f"reproducible mode: a frame group of {self.world} GPUs does not divide the {nc} GroupNorm chunks of "
+                             f"{HW}-pixel frames (frame groups of 2, 4 or 8 GPUs need H*W divisible by 8)")
+        return HW, nc, HW // nc
+
+    def gather_leaves(self, leaves: torch.Tensor, B: int, nc: int) -> torch.Tensor:
+        """This rank's leaves [(b, t, chunk_local), 32, 2] -> every rank's, in canonical [(b, t, chunk), 32, 2] order (exact copies)."""
+        P = self.world
+        ncl = nc // P
+        parts = leaves.new_empty((P,) + tuple(leaves.shape))
+        e0 = self._mark()
+        self.dist.all_gather_into_tensor(parts.view(-1), leaves.contiguous().view(-1), group=self.group)
+        self._done(e0)
+        return parts.view(P, B * self.T, ncl, 64).permute(1, 0, 2, 3).reshape(B * self.T * nc, 32, 2).contiguous()
+
+    def _groupnorm5d_leaves(self, x, B, gamma, beta, eps, silu, stat_rows):
+        from . import ops
+        HW, nc, rows_per_leaf = self.leaf_geometry(stat_rows)
+        leaves = self.gather_leaves(ops.groupnorm_leaves(x, rows_per_leaf), B, nc)
+        return ops.groupnorm_apply_leaves(x, B, leaves, stat_rows, gamma, beta, eps, silu)
 
     def gather_frames(self, y_local: torch.Tensor, T: int) -> torch.Tensor:
         """[B,C,T_local,H,W] per rank -> the full [B,C,T,H,W] on every rank (3.7 MB at the headline size)."""
@@ -157,6 +187,7 @@ class PeerFrameComm(FrameComm):
         self.device = torch.device(device)
         self.bmax = bmax
         self._bufs = {}            # name -> (own tensor, [device pointer of rank q's buffer as mapped here], capacity in elements)
+        self._leaves = None        # the same for the GroupNorm leaves of reproducible mode (float32, two halves of `capacity`)
         self._own_ptrs, self._peer_ptrs = [], []
         with torch.cuda.device(self.device):
             self.seq = torch.zeros(1, dtype=torch.int32, device=self.device)
@@ -244,12 +275,14 @@ class PeerFrameComm(FrameComm):
         own, ptrs, _ = self._buffer("sites" if to_sites else "frames", cap)
         dst = (C.c_void_p * P)(*ptrs)
         f0 = (C.c_int32 * (P + 1))(*([r[0] for r in self.ranges] + [self.T]))
-        _lib.check(self.lib.vc_peer_exchange(C.byref(self.c), h.data_ptr(), dst, int(to_sites), B, self.T, HW, Cc, f0, int(to_sites),
+        from . import ops
+        with_stats = to_sites and not ops.reproducible()          # reproducible mode takes its statistics from leaves
+        _lib.check(self.lib.vc_peer_exchange(C.byref(self.c), h.data_ptr(), dst, int(to_sites), B, self.T, HW, Cc, f0, int(with_stats),
                                              self.ws.data_ptr(), self.ws.numel() * 4, torch.cuda.current_stream().cuda_stream), "vc_peer_exchange")
         sent = h.numel() * 2
         self.bytes_moved += sent * (P - 1) // P if to_sites else sent - B * Tl * HWl * Cc * 2
         out = own[:out_rows * Cc].view(out_rows, Cc)
-        self._stats_of = out.data_ptr() if to_sites else None
+        self._stats_of = out.data_ptr() if with_stats else None
         return out
 
     def _to_sites(self, h: torch.Tensor, B: int, HW: int) -> torch.Tensor:
@@ -258,9 +291,40 @@ class PeerFrameComm(FrameComm):
     def _to_frames(self, t: torch.Tensor, B: int, HW: int) -> torch.Tensor:
         return self._exchange(t, B, HW, False)
 
+    def gather_leaves(self, leaves: torch.Tensor, B: int, nc: int) -> torch.Tensor:
+        """FrameComm.gather_leaves through peer memory: one kernel stores this rank's leaves into their canonical place of every rank's
+        leaf buffer and, after the rendezvous, copies the gathered array out (graph-capturable, no NCCL call)."""
+        import ctypes as C
+        from . import _lib
+        n = B * self.T * nc * 64
+        own, ptrs, cap = self._leaf_buffer(n)
+        out = torch.empty((B * self.T * nc, 32, 2), device=leaves.device, dtype=torch.float32)
+        e0 = self._mark()
+        _lib.check(self.lib.vc_peer_gather_leaves(C.byref(self.c), leaves.contiguous().data_ptr(), (C.c_void_p * self.world)(*ptrs), cap, B,
+                                                  self.T, nc, out.data_ptr(), torch.cuda.current_stream().cuda_stream), "vc_peer_gather_leaves")
+        self._done(e0)
+        return out
+
+    def _leaf_buffer(self, numel: int):
+        """float32 [2][cap] leaf buffer on every rank (collective growth, like _buffer) -> (own, peer pointers, cap)."""
+        ent = self._leaves
+        if ent is None or ent[2] < numel:
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("PeerFrameComm: the leaf buffer must grow during CUDA-graph capture; run one eager forward first")
+            torch.cuda.synchronize()
+            self.dist.barrier(group=self.group)
+            with torch.cuda.device(self.device):
+                own, ptrs = self._shared(2 * numel * 4, torch.float32)
+            ent = (own, ptrs, numel)
+            self._leaves = ent
+        return ent
+
     def groupnorm5d(self, x, B, gamma, beta, eps, silu, stat_rows, fresh: bool):
         import ctypes as C
         from . import _lib, ops
+        if ops.reproducible():
+            self._stats_of = None
+            return self._groupnorm5d_leaves(x, B, gamma, beta, eps, silu, stat_rows)
         stream = torch.cuda.current_stream().cuda_stream
         rows, Cc = x.shape
         if not (fresh and self._stats_of == x.data_ptr()):
@@ -303,7 +367,7 @@ class PeerFrameComm(FrameComm):
             self.lib.vc_peer_close(p)
         for p in self._own_ptrs:
             self.lib.vc_peer_free(p)
-        self._peer_ptrs, self._own_ptrs, self._bufs = [], [], {}
+        self._peer_ptrs, self._own_ptrs, self._bufs, self._leaves = [], [], {}, None
 
 
 class _ScatterPlan:
@@ -408,6 +472,16 @@ def shard_model(model, dist, rank: int, world: int, cfg_split: bool = True, peer
         device = next(unet.parameters()).device
     except StopIteration:
         device = None
+    from . import ops
+    modes = [None] * world
+    dist.all_gather_object(modes, ops.reproducible())
+    if len(set(modes)) != 1:
+        raise RuntimeError(f"shard_model: the ranks disagree on reproducible mode ({modes}); call viewcrafter_b200.set_reproducible() "
+                           f"or set VC_REPRODUCIBLE the same way on every rank")
+    P = world // 2 if (cfg_split and world % 2 == 0 and hasattr(model, "model")) else world
+    if ops.reproducible() and P not in (1, 2, 4, 8):
+        raise ValueError(f"shard_model: reproducible mode supports frame groups of 1, 2, 4 or 8 GPUs (they divide the GroupNorm chunks "
+                         f"of every frame); this layout puts {P} GPUs in a frame group")
     if peer is None:           # NVLink peer-memory kernels on CUDA (VC_PEER_COMM=0: NCCL collectives); the CPU double uses gloo
         import os
         peer = os.environ.get("VC_PEER_COMM", "1") != "0"

@@ -19,6 +19,7 @@ from __future__ import annotations
 
 import torch
 
+from . import ops
 from .ddim import DDIMSampler
 from .ddim_multiplecond import DDIMSampler as DDIMSampler_multicond
 
@@ -35,7 +36,22 @@ def get_latent_z(model, videos):
 def image_guided_synthesis(model, prompts, videos, noise_shape, n_samples=1, ddim_steps=50, ddim_eta=1.,
                            unconditional_guidance_scale=1.0, cfg_img=None, fs=None, text_input=False, multiple_cond_cfg=False,
                            timestep_spacing='uniform', guidance_rescale=0.0, condition_index=None, batch_cfg=True, cuda_graph=True,
-                           **kwargs):
+                           reproducible=None, **kwargs):
+    """reproducible: True / False switches viewcrafter_b200's reproducible mode (ops.set_reproducible) for this call and restores the
+    previous setting afterwards; None leaves the process setting as it is."""
+    if reproducible is None:
+        return _synthesis(model, prompts, videos, noise_shape, n_samples, ddim_steps, ddim_eta, unconditional_guidance_scale, cfg_img, fs,
+                          text_input, multiple_cond_cfg, timestep_spacing, guidance_rescale, condition_index, batch_cfg, cuda_graph, **kwargs)
+    prev = ops.set_reproducible(reproducible)
+    try:
+        return _synthesis(model, prompts, videos, noise_shape, n_samples, ddim_steps, ddim_eta, unconditional_guidance_scale, cfg_img, fs,
+                          text_input, multiple_cond_cfg, timestep_spacing, guidance_rescale, condition_index, batch_cfg, cuda_graph, **kwargs)
+    finally:
+        ops.set_reproducible(prev)
+
+
+def _synthesis(model, prompts, videos, noise_shape, n_samples, ddim_steps, ddim_eta, unconditional_guidance_scale, cfg_img, fs, text_input,
+               multiple_cond_cfg, timestep_spacing, guidance_rescale, condition_index, batch_cfg, cuda_graph, **kwargs):
     unet = getattr(getattr(model, "model", None), "diffusion_model", None)
     if cuda_graph and hasattr(unet, "enable_cuda_graph") and next(unet.parameters()).is_cuda:
         unet.enable_cuda_graph()              # the ~100 forwards of a clip share shapes, weights and context: capture once, replay

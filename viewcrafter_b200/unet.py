@@ -380,7 +380,7 @@ class UNetModel(nn.Module):
             Tg, HWl = (comm.T, HW // comm.world) if comm else (T, HW)
             n_tc, to_f = len(P["tconv"]), None
             for i, (g, be, w3, b3) in enumerate(P["tconv"]):
-                t = UNetModel._gn5d(t, B, g, be, 1e-5, True, comm, Tg * HW, fresh=(i == 0))   # statistics over (C/32, T, H, W)
+                t = UNetModel._gn5d(t, B, g, be, 1e-5, True, comm, Tg * HW, HW, fresh=(i == 0))   # statistics over (C/32, T, H, W)
                 last = i == n_tc - 1
                 to_f = comm.scatter_plan(False, B, HW, w3.shape[0] // 3) if (comm and last) else None
                 t = ops.conv_temporal(t, B, Tg, HWl, w3, bias=b3, res=ident if last else None, gn_out=comm is None, peer=to_f)
@@ -388,10 +388,12 @@ class UNetModel(nn.Module):
         return h2
 
     @staticmethod
-    def _gn5d(x, B, gamma, beta, eps, silu, comm, stat_rows, fresh=False):
-        """GroupNorm whose statistics span all frames (and, when sharded, all GPUs: [B,32,2] partial sums are exchanged --
-        riding on the layout switch when `fresh`, i.e. x is what comm.to_sites() just returned)."""
+    def _gn5d(x, B, gamma, beta, eps, silu, comm, stat_rows, hw, fresh=False):
+        """GroupNorm whose statistics span all frames of hw pixels (and, when sharded, all GPUs: [B,32,2] partial sums are exchanged --
+        riding on the layout switch when `fresh`, i.e. x is what comm.to_sites() just returned; canonical leaves in reproducible mode)."""
         if not comm:
+            if ops.reproducible():
+                return ops.groupnorm_canonical(x, B, hw, gamma, beta, eps, silu)
             return ops.groupnorm(x, B, gamma, beta, eps, silu)
         return comm.groupnorm5d(x, B, gamma, beta, eps, silu, stat_rows, fresh)
 
@@ -444,7 +446,7 @@ class UNetModel(nn.Module):
         Tg, HWl = (comm.T, HW // comm.world) if comm else (T, HW)
         t_in = h if pre_sites else (comm.to_sites(h, B, HW) if comm else h)
         fold = _LN_FOLD
-        x = ops.linear(UNetModel._gn5d(t_in, B, *P["gn"], 1e-6, False, comm, Tg * HW, fresh=True), P["in_w"], bias=P["in_b"], ln_out=fold)
+        x = ops.linear(UNetModel._gn5d(t_in, B, *P["gn"], 1e-6, False, comm, Tg * HW, HW, fresh=True), P["in_w"], bias=P["in_b"], ln_out=fold)
         x, st = x if fold else (x, None)
         for Q in P["blocks"]:
             for ln, wqkv, ow, ob in (("ln1", "qkv1", "o1_w", "o1_b"), ("ln2", "qkv2", "o2_w", "o2_b")):
@@ -554,7 +556,7 @@ class UNetModel(nn.Module):
     def _forward_graphed(self, x, timesteps, context, fs, kwargs):
         ver = ops.tensor_version(context)
         flags = tuple(sorted((k, bool(v)) for k, v in kwargs.items() if k == "cfg_shared_prefix"))
-        key = (tuple(x.shape), x.dtype, id(context), ver, fs is None, flags, id(self._comm))
+        key = (tuple(x.shape), x.dtype, id(context), ver, fs is None, flags, id(self._comm), ops.reproducible())
         e = self._graphs.get(key)
         if ver is None or (e is not None and e["ctx"] is not context):
             return self._forward_impl(x, timesteps, context, fs, kwargs)
