@@ -15,6 +15,8 @@ from typing import List
 
 import torch
 
+from .distributions import posterior_class
+
 
 def frame_ranges(T: int, world: int) -> List[tuple]:
     """Contiguous, as-even-as-possible split of T frames: 25 over 8 -> 4,3,3,3,3,3,3,3."""
@@ -445,6 +447,87 @@ class CfgComm:
         return buf[0, :rows[0]], buf[1, :rows[1]]
 
 
+# -- the VAE, frame-sharded over all ranks -----------------------------------------------------------------------------------------
+# The VAE is a 2-D network applied to every frame on its own (SURVEY.md 8(e)): frame f of the clip flattened as (b t) depends on
+# input frame f only.  Rank r encodes / decodes the frames frame_ranges(B*T, world)[r] and the shares are all-gathered; under the
+# CFG split too, since the VAE has no guidance branches.  The *_share functions compute one rank's share without a process group.
+
+def _flat_frames(x: torch.Tensor) -> torch.Tensor:
+    """[b, c, t, h, w] -> [(b t), c, h, w], the frame order of encode_first_stage / decode_core (ddpm3d.py:620-667)."""
+    b, c, t, h, w = x.shape
+    return x.permute(0, 2, 1, 3, 4).reshape(b * t, c, h, w)
+
+
+def vae_encode_share(model, videos: torch.Tensor, rank: int, world: int):
+    """Rank `rank`'s share of encoding videos [b, 3, t, H, W]: the fp32 posterior moments [n_r, 2*embed_dim, H/8, W/8] of its frames,
+    one first_stage_model.encode call per frame when model.perframe_ae, else one call for all of them (as encode_first_stage calls
+    it).  None for a rank without frames.  Draws no random numbers; vae_latents_from_moments samples the posterior."""
+    f0, f1 = frame_ranges(videos.shape[0] * videos.shape[2], world)[rank]
+    if f1 == f0:
+        return None
+    x = _flat_frames(videos)[f0:f1]
+    encode = model.first_stage_model.encode
+    if model.perframe_ae:
+        return torch.cat([encode(x[i:i + 1]).parameters for i in range(f1 - f0)], 0)
+    return encode(x).parameters
+
+
+def vae_latents_from_moments(model, moments: torch.Tensor, b: int, t: int) -> torch.Tensor:
+    """The moments of all b*t frames [(b t), 2*embed_dim, h, w] -> latents [b, embed_dim, t, h, w], sampled as encode_first_stage
+    samples them: one get_first_stage_encoding per frame when model.perframe_ae, else one over all frames.  The posterior draws
+    come from the CPU generator (distributions.py), so every rank replays all frames in order: each then leaves that generator in
+    the state a single process leaves it in."""
+    post = posterior_class()
+    if model.perframe_ae:
+        z = torch.cat([model.get_first_stage_encoding(post(moments[i:i + 1])).detach() for i in range(moments.shape[0])], 0)
+    else:
+        z = model.get_first_stage_encoding(post(moments)).detach()
+    return z.reshape(b, t, *z.shape[1:]).permute(0, 2, 1, 3, 4)
+
+
+def vae_decode_share(model, z: torch.Tensor, rank: int, world: int):
+    """Rank `rank`'s share of decode_first_stage(z) for latents z [b, c, t, h, w]: the model's own decode_first_stage on its frames
+    as one 4-D [n_r, c, h, w] tensor (so perframe_ae and decode_batch apply as the model defines them) -> [n_r, 3, H, W].
+    None for a rank without frames."""
+    f0, f1 = frame_ranges(z.shape[0] * z.shape[2], world)[rank]
+    if f1 == f0:
+        return None
+    return model.decode_first_stage(_flat_frames(z)[f0:f1])
+
+
+def gather_shares(comm: FrameComm, share, n: int, device, dtype) -> torch.Tensor:
+    """Every rank's share [n_r, C, H, W] of n frames (None on a rank without frames, which then contributes an empty share of
+    `dtype`) -> all n frames [n, C, H, W] on every rank: one all-gather padded to the largest share (FrameComm.gather_frames).
+    When n < world the ranks without frames first learn C, H, W from rank 0, which always holds a frame."""
+    comm.bind(n)
+    if n < comm.world:
+        dims = torch.tensor(list(share.shape[1:]) if share is not None else [0, 0, 0], dtype=torch.int64, device=device)
+        comm.dist.broadcast(dims, 0, group=comm.group)
+        if share is None:
+            share = torch.empty((0, *dims.tolist()), device=device, dtype=dtype)
+    return comm.gather_frames(share.permute(1, 0, 2, 3).unsqueeze(0), n)[0].transpose(0, 1)
+
+
+def vae_encode(model, videos: torch.Tensor) -> torch.Tensor:
+    """synthesis.get_latent_z sharded over the ranks of model._vae_comm (set by shard_model): videos [b, 3, t, H, W] -> latents
+    [b, embed_dim, t, H/8, W/8] on every rank.  The moments are all-gathered (fp32, 7.4 MB at 576x1024x25)."""
+    comm = model._vae_comm
+    b, t = videos.shape[0], videos.shape[2]
+    share = vae_encode_share(model, videos, comm.rank, comm.world)
+    moments = gather_shares(comm, share, b * t, videos.device, torch.float32).contiguous()
+    return vae_latents_from_moments(model, moments, b, t)
+
+
+def vae_decode(model, z: torch.Tensor) -> torch.Tensor:
+    """model.decode_first_stage(z) sharded over the ranks of model._vae_comm: latents [b, c, t, h, w] -> [b, 3, t, H, W] on every
+    rank, in the dtype decode_first_stage returns (the latents' for AutoencoderKL)."""
+    comm = model._vae_comm
+    b, t = z.shape[0], z.shape[2]
+    share = vae_decode_share(model, z, comm.rank, comm.world)
+    y = gather_shares(comm, share, b * t, z.device, z.dtype)
+    return y.reshape(b, t, *y.shape[1:]).permute(0, 2, 1, 3, 4)
+
+
 def _make_comm(dist, rank, world, group, device, peer: bool):
     if peer and world > 1 and device is not None and torch.device(device).type == "cuda":
         comm, err = None, None
@@ -466,7 +549,10 @@ def shard_model(model, dist, rank: int, world: int, cfg_split: bool = True, peer
 
     world even and cfg_split: 2-way CFG split x (world/2)-way frame sharding -- e.g. 8 GPUs = 2 x 4 with frames 7/6/6/6
     (ideal 7.1x) instead of 8-way frames 4/3x7 (ideal 6.25x).  Otherwise pure frame sharding.
-    Every rank must call this (it creates process groups collectively).  Returns the FrameComm (or None)."""
+    A model with a VAE (`first_stage_model`) also gets `model._vae_comm`, a FrameComm over all `world` ranks of the default group:
+    synthesis.get_latent_z and image_guided_synthesis then encode and decode the frames sharded over every rank (vae_encode,
+    vae_decode).  That adds no process group and no collective here.
+    Every rank must call this (it creates process groups collectively).  Returns the U-Net's FrameComm (or None)."""
     unet = model.model.diffusion_model if hasattr(model, "model") else model
     try:
         device = next(unet.parameters()).device
@@ -485,6 +571,8 @@ def shard_model(model, dist, rank: int, world: int, cfg_split: bool = True, peer
     if peer is None:           # NVLink peer-memory kernels on CUDA (VC_PEER_COMM=0: NCCL collectives); the CPU double uses gloo
         import os
         peer = os.environ.get("VC_PEER_COMM", "1") != "0"
+    if getattr(model, "first_stage_model", None) is not None:
+        model._vae_comm = FrameComm(dist, rank, world)
     if cfg_split and world % 2 == 0 and hasattr(model, "model"):
         P = world // 2
         frame_groups = [dist.new_group(list(range(b * P, (b + 1) * P))) for b in range(2)]

@@ -13,19 +13,29 @@ What differs from the reference, all parity-preserving (SURVEY.md App. C):
     iteration -- the cross-attention K/V projections are computed once per clip;
   * ``cuda_graph=True`` lets the viewcrafter_b200 U-Net replay its forward as one captured CUDA graph from the third call on
     (``UNetModel.enable_cuda_graph``): same kernels in the same order, ~1000 launches -> 1 per forward;
+  * on a model sharded by ``parallel.shard_model`` the VAE encode and decode run frame-sharded over all ranks (same latents, same
+    posterior draws in the same order, same decoded frames; INTEGRATION.md "Multi-GPU");
   * nothing else: conditioning tensors, ``x_T`` / per-step noise draws and the decode are the reference's, in its order.
 """
 from __future__ import annotations
 
 import torch
 
-from . import ops
+from . import ops, parallel
 from .ddim import DDIMSampler
 from .ddim_multiplecond import DDIMSampler as DDIMSampler_multicond
 
 
+def _vae_sharded(model) -> bool:
+    """True when parallel.shard_model gave the model a VAE communicator over more than one rank."""
+    return bool(getattr(model, "_vae_comm", None))
+
+
 def get_latent_z(model, videos):
-    """videos [b, c, t, h, w] -> latents [b, c', t, h/8, w/8] via per-frame encode_first_stage (diffusion_utils.py:110-115)."""
+    """videos [b, c, t, h, w] -> latents [b, c', t, h/8, w/8] via per-frame encode_first_stage (diffusion_utils.py:110-115).
+    On a model sharded by parallel.shard_model the frames are encoded over all ranks (parallel.vae_encode), same latents."""
+    if _vae_sharded(model):
+        return parallel.vae_encode(model, videos)
     b, c, t, h, w = videos.shape
     x = videos.permute(0, 2, 1, 3, 4).reshape(b * t, c, h, w)
     z = model.encode_first_stage(x)
@@ -100,5 +110,6 @@ def _synthesis(model, prompts, videos, noise_shape, n_samples, ddim_steps, ddim_
                                          unconditional_guidance_scale=unconditional_guidance_scale, unconditional_conditioning=uc,
                                          eta=ddim_eta, cfg_img=cfg_img, mask=None, x0=None, fs=fs,
                                          timestep_spacing=timestep_spacing, guidance_rescale=guidance_rescale, **kwargs)
-        batch_variants.append(model.decode_first_stage(samples))             # latent -> pixel space
+        # latent -> pixel space; on a sharded model every rank decodes its share of the frames (parallel.vae_decode)
+        batch_variants.append(parallel.vae_decode(model, samples) if _vae_sharded(model) else model.decode_first_stage(samples))
     return torch.stack(batch_variants).permute(1, 0, 2, 3, 4, 5)              # batch, variants, c, t, h, w
