@@ -15,6 +15,19 @@ import torch
 from . import ops, schedule
 
 
+def check_row_replay(opts: dict):
+    """Raise ValueError for a sample() option under which the rows of a batch cannot be sampled on their own with the batch's random
+    numbers (sample(_rng_rows=...), DDIMSampler.skip_sample_draws): noise_dropout > 0 and mask / x0 draw extra or data-dependent
+    numbers; x_T, timesteps and repeat_noise change what is drawn."""
+    bad = [name for name, on in (("noise_dropout > 0", opts.get("noise_dropout", 0.) > 0), ("mask", opts.get("mask") is not None),
+                                 ("x0", opts.get("x0") is not None), ("x_T", opts.get("x_T") is not None),
+                                 ("timesteps", opts.get("timesteps") is not None), ("repeat_noise", bool(opts.get("repeat_noise"))))
+           if on]
+    if bad:
+        raise ValueError(f"{bad[0]} is not supported when the rows of a batch are sampled on their own (replica groups, "
+                         f"parallel.shard_model(replicas=R > 1))")
+
+
 class DDIMSampler(object):
     def __init__(self, model, schedule="linear", batch_cfg: bool = False, **kwargs):
         super().__init__()
@@ -75,15 +88,21 @@ class DDIMSampler(object):
                quantize_x0=False, eta=0., mask=None, x0=None, temperature=1., noise_dropout=0., score_corrector=None,
                corrector_kwargs=None, verbose=True, schedule_verbose=False, x_T=None, log_every_t=100,
                unconditional_guidance_scale=1., unconditional_conditioning=None, precision=None, fs=None,
-               timestep_spacing='uniform', guidance_rescale=0.0, **kwargs):
+               timestep_spacing='uniform', guidance_rescale=0.0, _rng_rows=None, **kwargs):
+        """_rng_rows=(b0, b1): sample rows b0:b1 of a batch of `batch_size` on their own, with the random numbers the whole batch
+        would get: x_T and every step's noise are drawn at the full batch shape and rows b0:b1 are kept (the conditioning and fs
+        hold b1 - b0 rows).  Raises ValueError for the options whose draws it cannot replay (check_row_replay)."""
+        if _rng_rows is not None:
+            check_row_replay(dict(kwargs, noise_dropout=noise_dropout, mask=mask, x0=x0, x_T=x_T))
         if conditioning is not None:
             first = conditioning[list(conditioning.keys())[0]] if isinstance(conditioning, dict) else conditioning
             try:
                 cbs = first.shape[0]
             except AttributeError:
                 cbs = first[0].shape[0]
-            if cbs != batch_size:
-                print(f"Warning: Got {cbs} conditionings but batch-size is {batch_size}")
+            rows = batch_size if _rng_rows is None else _rng_rows[1] - _rng_rows[0]
+            if cbs != rows:
+                print(f"Warning: Got {cbs} conditionings but batch-size is {rows}")
         self.make_schedule(ddim_num_steps=S, ddim_discretize=timestep_spacing, ddim_eta=eta, verbose=schedule_verbose)
         if len(shape) == 3:
             size = (batch_size, *shape)
@@ -96,19 +115,30 @@ class DDIMSampler(object):
                                   temperature=temperature, score_corrector=score_corrector, corrector_kwargs=corrector_kwargs,
                                   x_T=x_T, log_every_t=log_every_t, unconditional_guidance_scale=unconditional_guidance_scale,
                                   unconditional_conditioning=unconditional_conditioning, verbose=verbose, precision=precision,
-                                  fs=fs, guidance_rescale=guidance_rescale, **kwargs)
+                                  fs=fs, guidance_rescale=guidance_rescale, _rng_rows=_rng_rows, **kwargs)
+
+    def skip_sample_draws(self, S, size, device, timestep_spacing="uniform"):
+        """Consume from the generator of `device` exactly what one sample(S=S, timestep_spacing=...) call at the batch shape `size`
+        consumes when check_row_replay accepts its options: x_T (ddim_sampling), then one noise tensor per step (_step_noise)."""
+        for _ in range(1 + len(schedule.ddim_timesteps(timestep_spacing, S, self.ddpm_num_timesteps))):
+            torch.randn(size, device=device)
 
     @torch.no_grad()
     def ddim_sampling(self, cond, shape, x_T=None, ddim_use_original_steps=False, callback=None, timesteps=None,
                       quantize_denoised=False, mask=None, x0=None, img_callback=None, log_every_t=100, temperature=1.,
                       noise_dropout=0., score_corrector=None, corrector_kwargs=None, unconditional_guidance_scale=1.,
-                      unconditional_conditioning=None, verbose=True, precision=None, fs=None, guidance_rescale=0.0, **kwargs):
+                      unconditional_conditioning=None, verbose=True, precision=None, fs=None, guidance_rescale=0.0, _rng_rows=None,
+                      **kwargs):
         if ddim_use_original_steps:
             # the reference's own branch reads self.ddim_sigmas_for_original_num_steps, which its make_schedule never defines (ddim.py:248)
             raise NotImplementedError("viewcrafter_b200.DDIMSampler: ddim_use_original_steps is not implemented (it fails in the reference too)")
         device = self._device()
         b = shape[0]
         img = torch.randn(shape, device=device) if x_T is None else x_T
+        rng_batch = None
+        if _rng_rows is not None:                           # sample(_rng_rows=...): keep rows b0:b1 of the batch's draws (_step_noise too)
+            img, b = img[_rng_rows[0]:_rng_rows[1]].contiguous(), _rng_rows[1] - _rng_rows[0]
+            rng_batch = (shape[0], _rng_rows[0])
         if precision is not None and int(precision) == 16:
             img = img.to(dtype=torch.float16)               # ddim.py:154-156: only x_T is rounded; every later latent is fp32 again
         steps = self.ddim_timesteps
@@ -130,7 +160,7 @@ class DDIMSampler(object):
                                               score_corrector=score_corrector, corrector_kwargs=corrector_kwargs,
                                               unconditional_guidance_scale=unconditional_guidance_scale,
                                               unconditional_conditioning=unconditional_conditioning, mask=mask, x0=x0, fs=fs,
-                                              guidance_rescale=guidance_rescale, _step=int(step), **kwargs)
+                                              guidance_rescale=guidance_rescale, _step=int(step), _rng_batch=rng_batch, **kwargs)
             if callback:
                 callback(i)
             if img_callback:
@@ -190,7 +220,8 @@ class DDIMSampler(object):
     def p_sample_ddim(self, x, c, t, index, repeat_noise=False, use_original_steps=False, quantize_denoised=False,
                       temperature=1., noise_dropout=0., score_corrector=None, corrector_kwargs=None,
                       unconditional_guidance_scale=1., unconditional_conditioning=None, uc_type=None,
-                      conditional_guidance_scale_temporal=None, mask=None, x0=None, guidance_rescale=0.0, _step=None, **kwargs):
+                      conditional_guidance_scale_temporal=None, mask=None, x0=None, guidance_rescale=0.0, _step=None, _rng_batch=None,
+                      **kwargs):
         self._check_step_options(use_original_steps, quantize_denoised, score_corrector)
         step = int(t[0].item()) if _step is None else _step
         if unconditional_conditioning is None or unconditional_guidance_scale == 1.:
@@ -201,7 +232,7 @@ class DDIMSampler(object):
             v_c, v_u = self._apply_both(x, t, c, unconditional_conditioning, kwargs)
         sc = self.step_scalars(index, step)
         sc["cfg_scale"], sc["guidance_rescale"] = float(unconditional_guidance_scale), float(guidance_rescale)
-        noise = self._step_noise(x, repeat_noise, temperature, noise_dropout)
+        noise = self._step_noise(x, repeat_noise, temperature, noise_dropout, _rng_batch)
         return self._fused_update(x, v_c, v_u, noise, sc)
 
     # -- pieces shared with the three-way sampler (ddim_multiplecond.py) ------------------------------------------------
@@ -217,10 +248,14 @@ class DDIMSampler(object):
             raise AssertionError("not implemented")          # ddim.py:239-241 asserts parameterization == 'eps' before using a score corrector
 
     @staticmethod
-    def _step_noise(x, repeat_noise, temperature, noise_dropout):
-        """noise_like * temperature, then dropout (ddim.py:275-277; the scalar sigma_t is applied by the fused update, which commutes with both)."""
+    def _step_noise(x, repeat_noise, temperature, noise_dropout, rng_batch=None):
+        """noise_like * temperature, then dropout (ddim.py:275-277; the scalar sigma_t is applied by the fused update, which commutes with both).
+        rng_batch=(B, b0) (sample(_rng_rows=...)): x holds rows b0: of a batch of B; the noise is drawn for the batch and those rows kept."""
         shape = (1, *x.shape[1:]) if repeat_noise else x.shape
-        noise = torch.randn(shape, device=x.device)                      # same draw as lvdm/common.py:31-34
+        if rng_batch is not None:
+            noise = torch.randn((rng_batch[0], *x.shape[1:]), device=x.device)[rng_batch[1]:rng_batch[1] + x.shape[0]]
+        else:
+            noise = torch.randn(shape, device=x.device)                  # same draw as lvdm/common.py:31-34
         if repeat_noise:
             noise = noise.repeat(x.shape[0], *((1,) * (x.dim() - 1)))
         if temperature != 1.:

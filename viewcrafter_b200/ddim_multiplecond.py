@@ -34,7 +34,7 @@ class DDIMSampler(_TwoWaySampler):
     def p_sample_ddim(self, x, c, t, index, repeat_noise=False, use_original_steps=False, quantize_denoised=False,
                       temperature=1., noise_dropout=0., score_corrector=None, corrector_kwargs=None,
                       unconditional_guidance_scale=1., unconditional_conditioning=None, uc_type=None, cfg_img=None,
-                      mask=None, x0=None, guidance_rescale=0.0, _step=None, **kwargs):
+                      mask=None, x0=None, guidance_rescale=0.0, _step=None, _rng_batch=None, **kwargs):
         self._check_step_options(use_original_steps, quantize_denoised, score_corrector)
         if cfg_img is None:
             cfg_img = unconditional_guidance_scale
@@ -50,7 +50,7 @@ class DDIMSampler(_TwoWaySampler):
             v_c, v_u, v_i = self._apply_three(x, t, c, unconditional_conditioning, uc_img, kwargs)
         sc = self.step_scalars(index, step)
         sc["cfg_scale"], sc["guidance_rescale"] = float(unconditional_guidance_scale), float(guidance_rescale)
-        noise = self._step_noise(x, repeat_noise, temperature, noise_dropout)
+        noise = self._step_noise(x, repeat_noise, temperature, noise_dropout, _rng_batch)
         return self._fused_update(x, v_c, v_u, noise, sc, v_uncond_img=v_i, cfg_img=float(cfg_img))
 
     def _apply_three(self, x, t, c, uc, uc_img, kwargs):

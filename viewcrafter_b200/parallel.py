@@ -528,6 +528,32 @@ def vae_decode(model, z: torch.Tensor) -> torch.Tensor:
     return y.reshape(b, t, *y.shape[1:]).permute(0, 2, 1, 3, 4)
 
 
+class Replicas:
+    """shard_model(replicas=R): the world cut into R groups of world / R consecutive ranks, each running whole outputs of a synthesis
+    call.  synthesis.image_guided_synthesis numbers the outputs j = k * B + b (sample k, clip b) and runs job j on group j % R; a group
+    runs its jobs in increasing j.  `index` is this rank's group; collectives go over the default group (the whole world)."""
+
+    def __init__(self, dist, index: int, count: int, world: int):
+        self.dist, self.index, self.count, self.world = dist, index, count, world
+        self.size = world // count
+
+    def jobs(self, n_jobs: int) -> List[int]:
+        """The jobs of this rank's group, in the order it runs them (none when n_jobs <= index: the group is idle)."""
+        return list(range(self.index, n_jobs, self.count))
+
+    def gather_jobs(self, mine: List[torch.Tensor], n_jobs: int, shape, device) -> torch.Tensor:
+        """This group's job results (fp32 [1, *shape] each, in the order of jobs()) -> all n_jobs results [n_jobs, *shape] in job order, on
+        every rank: one all-gather over the world, padded to the largest group's job count (idle groups send padding only).  Every rank
+        of a group holds the same results; the first rank's are taken."""
+        m = -(-n_jobs // self.count)
+        send = torch.zeros((m, *shape), device=device, dtype=torch.float32)
+        for i, t in enumerate(mine):
+            send[i] = t[0]
+        parts = send.new_empty((self.world, m, *shape))
+        self.dist.all_gather_into_tensor(parts.view(-1), send.view(-1))
+        return torch.stack([parts[(j % self.count) * self.size, j // self.count] for j in range(n_jobs)])
+
+
 def _make_comm(dist, rank, world, group, device, peer: bool):
     if peer and world > 1 and device is not None and torch.device(device).type == "cuda":
         comm, err = None, None
@@ -544,11 +570,14 @@ def _make_comm(dist, rank, world, group, device, peer: bool):
     return FrameComm(dist, rank, world, group)
 
 
-def shard_model(model, dist, rank: int, world: int, cfg_split: bool = True, peer: bool = None):
+def shard_model(model, dist, rank: int, world: int, cfg_split: bool = True, peer: bool = None, replicas: int = 1):
     """Distribute the denoise step over `world` ranks (weights stay replicated: 2.9 GB fp16 per GPU).
 
     world even and cfg_split: 2-way CFG split x (world/2)-way frame sharding -- e.g. 8 GPUs = 2 x 4 with frames 7/6/6/6
     (ideal 7.1x) instead of 8-way frames 4/3x7 (ideal 6.25x).  Otherwise pure frame sharding.
+    replicas=R: the world is cut into R groups of G = world / R consecutive ranks and the layout above applies inside each group, to
+    G ranks; a group of one rank has no communicator and runs the one-GPU path.  The model gets `model._replicas` (Replicas), and
+    synthesis.image_guided_synthesis then runs the samples and clips of one call concurrently, one whole output per group at a time.
     A model with a VAE (`first_stage_model`) also gets `model._vae_comm`, a FrameComm over all `world` ranks of the default group:
     synthesis.get_latent_z and image_guided_synthesis then encode and decode the frames sharded over every rank (vae_encode,
     vae_decode).  That adds no process group and no collective here.
@@ -560,11 +589,18 @@ def shard_model(model, dist, rank: int, world: int, cfg_split: bool = True, peer
         device = None
     from . import ops
     modes = [None] * world
-    dist.all_gather_object(modes, ops.reproducible())
-    if len(set(modes)) != 1:
-        raise RuntimeError(f"shard_model: the ranks disagree on reproducible mode ({modes}); call viewcrafter_b200.set_reproducible() "
-                           f"or set VC_REPRODUCIBLE the same way on every rank")
-    P = world // 2 if (cfg_split and world % 2 == 0 and hasattr(model, "model")) else world
+    dist.all_gather_object(modes, (ops.reproducible(), replicas))
+    if len(set(m for m, _ in modes)) != 1:
+        raise RuntimeError(f"shard_model: the ranks disagree on reproducible mode ({[m for m, _ in modes]}); call "
+                           f"viewcrafter_b200.set_reproducible() or set VC_REPRODUCIBLE the same way on every rank")
+    if len(set(r for _, r in modes)) != 1:
+        raise ValueError(f"shard_model: the ranks disagree on replicas ({[r for _, r in modes]})")
+    if not isinstance(replicas, int) or replicas < 1 or world % replicas != 0:
+        raise ValueError(f"shard_model: replicas must be a positive integer that divides the world size {world}, got {replicas!r}")
+    G = world // replicas                                  # ranks per replica group; the group of this rank starts at rank `off`
+    g, off = rank // G, rank // G * G
+    split = cfg_split and G % 2 == 0 and hasattr(model, "model")
+    P = G // 2 if split else G
     if ops.reproducible() and P not in (1, 2, 4, 8):
         raise ValueError(f"shard_model: reproducible mode supports frame groups of 1, 2, 4 or 8 GPUs (they divide the GroupNorm chunks "
                          f"of every frame); this layout puts {P} GPUs in a frame group")
@@ -573,13 +609,22 @@ def shard_model(model, dist, rank: int, world: int, cfg_split: bool = True, peer
         peer = os.environ.get("VC_PEER_COMM", "1") != "0"
     if getattr(model, "first_stage_model", None) is not None:
         model._vae_comm = FrameComm(dist, rank, world)
-    if cfg_split and world % 2 == 0 and hasattr(model, "model"):
-        P = world // 2
-        frame_groups = [dist.new_group(list(range(b * P, (b + 1) * P))) for b in range(2)]
-        pair_groups = [dist.new_group([i, i + P]) for i in range(P)]
-        branch, r = rank // P, rank % P
+    if replicas > 1:
+        model._replicas = Replicas(dist, g, replicas, world)
+    if split:
+        # every rank creates every group's process groups, in the same order (new_group is collective over the default group)
+        groups = [([dist.new_group(list(range(o + b * P, o + (b + 1) * P))) for b in range(2)],
+                   [dist.new_group([o + i, o + i + P]) for i in range(P)]) for o in range(0, world, G)]
+        frame_groups, pair_groups = groups[g]
+        branch, r = (rank - off) // P, (rank - off) % P
         model._cfg = CfgComm(dist, branch, pair_groups[r])
         unet._comm = _make_comm(dist, r, P, frame_groups[branch], device, peer) if P > 1 else None
         return unet._comm
-    unet._comm = _make_comm(dist, rank, world, None, device, peer)
+    if replicas == 1:
+        unet._comm = _make_comm(dist, rank, world, None, device, peer)
+    elif G == 1:
+        unet._comm = None
+    else:
+        groups = [dist.new_group(list(range(o, o + G))) for o in range(0, world, G)]
+        unet._comm = _make_comm(dist, rank - off, G, groups[g], device, peer)
     return unet._comm

@@ -15,6 +15,8 @@ What differs from the reference, all parity-preserving (SURVEY.md App. C):
     (``UNetModel.enable_cuda_graph``): same kernels in the same order, ~1000 launches -> 1 per forward;
   * on a model sharded by ``parallel.shard_model`` the VAE encode and decode run frame-sharded over all ranks (same latents, same
     posterior draws in the same order, same decoded frames; INTEGRATION.md "Multi-GPU");
+  * on a model sharded with ``shard_model(replicas=R > 1)`` the ``n_samples`` x batch outputs run concurrently on R GPU groups, each
+    with the random numbers the single process draws for it, and are decoded together over all ranks (``_sample_on_replicas``);
   * nothing else: conditioning tensors, ``x_T`` / per-step noise draws and the decode are the reference's, in its order.
 """
 from __future__ import annotations
@@ -22,7 +24,7 @@ from __future__ import annotations
 import torch
 
 from . import ops, parallel
-from .ddim import DDIMSampler
+from .ddim import DDIMSampler, check_row_replay
 from .ddim_multiplecond import DDIMSampler as DDIMSampler_multicond
 
 
@@ -62,6 +64,8 @@ def image_guided_synthesis(model, prompts, videos, noise_shape, n_samples=1, ddi
 
 def _synthesis(model, prompts, videos, noise_shape, n_samples, ddim_steps, ddim_eta, unconditional_guidance_scale, cfg_img, fs, text_input,
                multiple_cond_cfg, timestep_spacing, guidance_rescale, condition_index, batch_cfg, cuda_graph, **kwargs):
+    if getattr(model, "_replicas", None) is not None:
+        check_row_replay(kwargs)                          # before any collective, on every rank alike
     unet = getattr(getattr(model, "model", None), "diffusion_model", None)
     if cuda_graph and hasattr(unet, "enable_cuda_graph") and next(unet.parameters()).is_cuda:
         unet.enable_cuda_graph()              # the ~100 forwards of a clip share shapes, weights and context: capture once, replay
@@ -104,12 +108,66 @@ def _synthesis(model, prompts, videos, noise_shape, n_samples, ddim_steps, ddim_
     else:
         kwargs.update({"unconditional_conditioning_img_nonetext": None})
 
+    options = dict(S=ddim_steps, batch_size=batch_size, shape=noise_shape[1:], verbose=False,
+                   unconditional_guidance_scale=unconditional_guidance_scale, eta=ddim_eta, cfg_img=cfg_img, mask=None, x0=None,
+                   timestep_spacing=timestep_spacing, guidance_rescale=guidance_rescale, **kwargs)
+    replicas = getattr(model, "_replicas", None)
+    if replicas is not None:
+        return _sample_on_replicas(model, replicas, ddim_sampler, cond, uc, fs, n_samples, options)
     batch_variants = []
     for _ in range(n_samples):
-        samples, _ = ddim_sampler.sample(S=ddim_steps, conditioning=cond, batch_size=batch_size, shape=noise_shape[1:], verbose=False,
-                                         unconditional_guidance_scale=unconditional_guidance_scale, unconditional_conditioning=uc,
-                                         eta=ddim_eta, cfg_img=cfg_img, mask=None, x0=None, fs=fs,
-                                         timestep_spacing=timestep_spacing, guidance_rescale=guidance_rescale, **kwargs)
+        samples, _ = ddim_sampler.sample(conditioning=cond, unconditional_conditioning=uc, fs=fs, **options)
         # latent -> pixel space; on a sharded model every rank decodes its share of the frames (parallel.vae_decode)
         batch_variants.append(parallel.vae_decode(model, samples) if _vae_sharded(model) else model.decode_first_stage(samples))
     return torch.stack(batch_variants).permute(1, 0, 2, 3, 4, 5)              # batch, variants, c, t, h, w
+
+
+def _rows(conds, b):
+    """Row b of the conditioning dicts `conds` (None stays None).  Every tensor is sliced once, so entries that share a tensor (the
+    c_concat of all branches) share its slice: the shared CFG prefix, the U-Net's K/V cache and its graph key rely on that identity."""
+    memo = {}
+
+    def row(t):
+        if id(t) not in memo:
+            memo[id(t)] = t[b:b + 1]
+        return memo[id(t)]
+    return [None if c is None else {k: [row(t) for t in v] for k, v in c.items()} for c in conds]
+
+
+def _sample_on_replicas(model, replicas, sampler, cond, uc, fs, n_samples, options):
+    """The sampling and decode of image_guided_synthesis on a model sharded with shard_model(replicas=R > 1).  The n_samples x B
+    outputs are independent jobs j = k * B + b (sample k, clip b); group j % R runs job j as rows (b, b + 1) of sample k's batch
+    (DDIMSampler.sample(_rng_rows=...)), with the random numbers a single process draws for that batch.  The job latents are gathered
+    over the world and all n_samples * B clips are decoded in one parallel.vae_decode over all ranks.  Returns [B, n_samples, c, t, h, w]
+    on every rank, and leaves the device generator in the state a single process leaves it in."""
+    B = options["batch_size"]
+    n_jobs = n_samples * B
+    mine = replicas.jobs(n_jobs)
+    device = sampler._device()
+    if device.type == "cuda":
+        get_state, set_state = (lambda: torch.cuda.get_rng_state(device)), (lambda s: torch.cuda.set_rng_state(s, device))
+    else:
+        get_state, set_state = torch.get_rng_state, torch.set_rng_state
+    # a single process draws x_T and every step's noise of sample 0, then of sample 1, ...: walk that stream once, keeping the
+    # generator state at the start of every sample this group has a job in
+    starts = {}
+    for k in range(n_samples):
+        if any(j // B == k for j in mine):
+            starts[k] = get_state()
+        sampler.skip_sample_draws(options["S"], (B, *options["shape"]), device, options["timestep_spacing"])
+    end = get_state()
+    clips, latents = {}, []
+    for j in mine:
+        k, b = divmod(j, B)
+        if b not in clips:                 # one sampler per clip: its stacked conditioning (and the U-Net graph) is reused by every job
+            c, u, u2 = _rows((cond, uc, options["unconditional_conditioning_img_nonetext"]), b)
+            clips[b] = (type(sampler)(model, batch_cfg=sampler.batch_cfg),
+                        dict(options, conditioning=c, unconditional_conditioning=u, unconditional_conditioning_img_nonetext=u2, fs=fs[b:b + 1]))
+        smp, kw = clips[b]
+        set_state(starts[k])
+        z, _ = smp.sample(_rng_rows=(b, b + 1), **kw)
+        latents.append(z)
+    set_state(end)
+    z = replicas.gather_jobs(latents, n_jobs, tuple(options["shape"]), device)
+    y = parallel.vae_decode(model, z) if _vae_sharded(model) else model.decode_first_stage(z)
+    return y.reshape(n_samples, B, *y.shape[1:]).permute(1, 0, 2, 3, 4, 5)
