@@ -98,7 +98,8 @@ struct GemmParams {
   int gn_hp;               //   [m_tile * 4 + quadrant][N / 32][4]; a chunk is cut at the boundaries of gn_sub = 2 * gn_hp channel sub-groups
   int gn_nchunks;          //   (4 pieces: first partial, two whole, last partial / whole) -- see gn_part_accumulate and norm.cu: gn_part_finalize_kernel
   int out_tma;           // fp16 output written by TMA stores from per-warp staging tiles (full-line, LSU-free)
-  int vec_ok;            // rows are 32-byte aligned: the 256-bit epilogue path may be used
+  int vec_ok;            // output rows are 32-byte aligned: whole 32-column chunks of a non-TMA output are stored as 256-bit vectors
+  int res_vec;           // residual rows are 32-byte aligned: whole 32-column chunks of the residual are loaded as 256-bit vectors
   GemmPeer peer;         // output scattered to the ranks of the frame group (mode != 0: `out` itself is not written)
 };
 
@@ -198,8 +199,10 @@ __device__ __forceinline__ void peer_scatter32(const GemmParams& p, const EpiTil
   }
 }
 
-// store 32 consecutive output columns of this thread's row (fp16 or fp32), vector path or predicated scalar path
-__device__ __forceinline__ void epi_store32(const GemmParams& p, const EpiTile& t, int col0, int n_out, float (&f)[32], bool res_scalar,
+// store 32 consecutive output columns of this thread's row (fp16 or fp32): TMA store, vector path or predicated scalar path.
+// f holds the final values (bias and residual already added by epi_chunk): every path rounds the same fp32 values once,
+// round-to-nearest, so the fp16 output does not depend on which path its pointer and pitch select.
+__device__ __forceinline__ void epi_store32(const GemmParams& p, const EpiTile& t, int col0, int n_out, float (&f)[32],
                                             uint8_t* stage, int lane) {
   if (p.out_tma) {
     // Stage the warp's 32 x 32 fp16 tile in shared memory (64B-swizzled rows: conflict-free 16-byte stores) and let the TMA
@@ -242,10 +245,8 @@ __device__ __forceinline__ void epi_store32(const GemmParams& p, const EpiTile& 
 #pragma unroll
     for (int e = 0; e < 32; ++e) {
       if (col0 + e < n_out) {
-        float v = f[e];
-        if (res_scalar) v += __half2float(p.res[t.orow * p.ldr + col0 + e]);
-        if (p.out_f32) p.out_f32[t.orow * p.ldo + col0 + e] = v;
-        else p.out[t.orow * p.ldo + col0 + e] = __float2half_rn(v);
+        if (p.out_f32) p.out_f32[t.orow * p.ldo + col0 + e] = f[e];
+        else p.out[t.orow * p.ldo + col0 + e] = __float2half_rn(f[e]);
       }
     }
   }
@@ -330,9 +331,9 @@ __device__ __forceinline__ void gn_part_accumulate(const GemmParams& p, const Ep
 // One 32-column chunk of this thread's row: folded LayerNorm, bias, residual, output statistics, store.
 // nb: first column in the accumulator's N space (bias / LayerNorm column sums / residual / statistics), col0: first output column.
 // plain: the values are final already (GEGLU, computed on the fragments), only statistics-free storing remains.
+// The residual is added here, in registers, whatever the store path: the statistics and every store path see the same values.
 __device__ __forceinline__ void epi_chunk(const GemmParams& p, const EpiTile& t, int nb, int col0, int n_out, bool plain, float (&f)[32],
                                           uint8_t* stage, int lane) {
-  bool res_vec = false;
   if (!plain) {
     if (p.ln_stats) {                              // folded LayerNorm (host guarantees N % 32 == 0)
       const float2 ln = t.row_ok ? __ldg(reinterpret_cast<const float2*>(p.ln_stats) + t.orow) : make_float2(0.f, 1.f);
@@ -356,18 +357,26 @@ __device__ __forceinline__ void epi_chunk(const GemmParams& p, const EpiTile& t,
           if (nb + e < p.N) f[e] += __ldg(t.bias + nb + e);
       }
     }
-    res_vec = p.res != nullptr && p.vec_ok && t.row_ok && nb + 32 <= p.N;
-    if (res_vec) {
-      const uint4* rp = reinterpret_cast<const uint4*>(p.res + t.orow * p.ldr + nb);   // plain loads: res may alias out (in-place residual)
+    // plain loads, not __ldg: res may alias out (in-place residual)
+    if (p.res != nullptr && t.row_ok) {
+      if (p.res_vec && nb + 32 <= p.N) {
+        const uint4* rp = reinterpret_cast<const uint4*>(p.res + t.orow * p.ldr + nb);
 #pragma unroll
-      for (int h = 0; h < 4; ++h) {
-        const uint4 u = rp[h];
-        const __half2* r2 = reinterpret_cast<const __half2*>(&u);
+        for (int h = 0; h < 4; ++h) {
+          const uint4 u = rp[h];
+          const __half2* r2 = reinterpret_cast<const __half2*>(&u);
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float2 r = __half22float2(r2[e]);
-          f[h * 8 + 2 * e] += r.x; f[h * 8 + 2 * e + 1] += r.y;
+          for (int e = 0; e < 4; ++e) {
+            const float2 r = __half22float2(r2[e]);
+            f[h * 8 + 2 * e] += r.x; f[h * 8 + 2 * e + 1] += r.y;
+          }
         }
+      } else {
+        // ragged N tail / residual rows not 32-byte aligned: predicated scalar loads
+        const __half* rp = p.res + t.orow * p.ldr + nb;
+#pragma unroll
+        for (int e = 0; e < 32; ++e)
+          if (nb + e < p.N) f[e] += __half2float(rp[e]);
       }
     }
     if (p.ln_part) {                               // LayerNorm statistics of the OUTPUT row, as stored (fp16-rounded)
@@ -382,7 +391,7 @@ __device__ __forceinline__ void epi_chunk(const GemmParams& p, const EpiTile& t,
     }
     if (p.gn_part) gn_part_accumulate(p, t, nb, f, lane);
   }
-  epi_store32(p, t, col0, n_out, f, !plain && p.res != nullptr && !res_vec, stage, lane);
+  epi_store32(p, t, col0, n_out, f, stage, lane);
 }
 #endif  // __CUDACC__
 

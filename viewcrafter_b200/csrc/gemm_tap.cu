@@ -273,6 +273,10 @@ int gemm_tap(const GemmDesc& d, cudaStream_t stream) {
     set_error("gemm_tap: operands must be 16-byte aligned");
     return VC_ERR_ARG;
   }
+  // the epilogue reads the bias as float4: every bias row (row z / bias_z_div starts at bias + that * N) must be 16-byte aligned
+  VC_REQUIRE(!d.bias || (reinterpret_cast<uintptr_t>(d.bias) & 15) == 0, "gemm_tap: bias must be 16-byte aligned");
+  VC_REQUIRE(!d.bias || d.bias_z_div <= 0 || d.N % 4 == 0, "gemm_tap: per-z bias rows (bias_z_div=%d) need N %% 4 == 0 (N=%d)",
+             d.bias_z_div, d.N);
   const void* optr = d.out_f32 ? (const void*)d.out_f32 : (const void*)d.out;
   const int esz = d.out_f32 ? 4 : 2;
 
@@ -336,10 +340,10 @@ int gemm_tap(const GemmDesc& d, cudaStream_t stream) {
              "gemm_tap: GroupNorm partial sums need an fp16 output with N %% 32 == 0 and N %% gn_sub == 0 (gn_sub 10 or 8)");
   p.gn_part = reinterpret_cast<float2*>(d.gn_part); p.gn_hp = d.gn_sub / 2; p.gn_nchunks = d.N / 32;
   // vector epilogue accesses need 32-byte aligned rows (true for every activation on the U-Net / VAE path); anything
-  // else (odd pitches, the 4- and 3-channel output convs) takes the predicated scalar path inside the kernel
-  const bool o_al = ((reinterpret_cast<uintptr_t>(optr) & 31) == 0) && ((long long)d.ldo * esz) % 32 == 0;
-  const bool r_al = !d.res || (((reinterpret_cast<uintptr_t>(d.res) & 31) == 0) && ((long long)d.ldr * 2) % 32 == 0);
-  p.vec_ok = (o_al && r_al) ? 1 : 0;
+  // else (odd pitches, the 4- and 3-channel output convs) takes the predicated scalar path inside the kernel.  The output
+  // and the residual are judged separately: the residual is added in registers before any store path runs.
+  p.vec_ok = ((reinterpret_cast<uintptr_t>(optr) & 31) == 0) && ((long long)d.ldo * esz) % 32 == 0 ? 1 : 0;
+  p.res_vec = d.res && ((reinterpret_cast<uintptr_t>(d.res) & 31) == 0) && ((long long)d.ldr * 2) % 32 == 0 ? 1 : 0;
   {
     // TMA-store epilogue: fp16 output whose width is whole 32-column chunks and whose rows are 16-byte aligned
     const int n_out = d.geglu ? d.N / 2 : d.N;

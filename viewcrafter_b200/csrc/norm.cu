@@ -236,6 +236,8 @@ __global__ void __launch_bounds__(512, 2) gn_fused_kernel(const __half* __restri
 static int gn_geometry(GnGeom& g, const __half* x1, int C1, const __half* x2, int C2, int samples, long long rows_per_sample) {
   const int C = C1 + (x2 ? C2 : 0);
   VC_REQUIRE(x1, "groupnorm: null pointer");
+  VC_REQUIRE(((reinterpret_cast<uintptr_t>(x1) | reinterpret_cast<uintptr_t>(x2)) & 15) == 0,
+             "groupnorm: inputs must be 16-byte aligned (rows are read as 8-channel vectors)");
   VC_REQUIRE(C % 32 == 0 && C1 % 8 == 0 && (!x2 || C2 % 8 == 0) && C <= 4096, "groupnorm: unsupported channels C1=%d C2=%d", C1, C2);
   VC_REQUIRE(samples >= 1 && rows_per_sample >= 1, "groupnorm: empty input");
   g.C = C; g.C1 = C1; g.C2 = x2 ? C2 : 0;
@@ -617,6 +619,8 @@ int layernorm_rows(const __half* x, long long rows, int C, const float* gamma, c
                    cudaStream_t stream) {
   VC_REQUIRE(x && out && gamma && beta, "layernorm: null pointer");
   VC_REQUIRE(C % 8 == 0 && C <= 2048 && rows > 0, "layernorm: unsupported C=%d rows=%lld", C, rows);
+  VC_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out)) & 15) == 0,
+             "layernorm: x and out must be 16-byte aligned (rows are read and written as 8-channel vectors)");
   const int wpb = 8;
   long long blocks = (rows + 2 * wpb - 1) / (2 * wpb);
   const long long cap = (long long)sm_count() * 8;              // 8 x 256 threads = 64 warps per SM
@@ -785,6 +789,7 @@ int layernorm_stats(const __half* x, long long rows, int C, float eps, float* st
   VC_REQUIRE(x && stats, "layernorm_stats: null pointer");
   VC_REQUIRE(C % 8 == 0 && C <= 8192 && rows > 0, "layernorm_stats: unsupported C=%d rows=%lld", C, rows);
   VC_REQUIRE((reinterpret_cast<uintptr_t>(stats) & 7) == 0, "layernorm_stats: stats must be 8-byte aligned");
+  VC_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "layernorm_stats: x must be 16-byte aligned (rows are read as 8-channel vectors)");
   const int wpb = 8;
   long long blocks = (rows + 4 * wpb - 1) / (4 * wpb);
   const long long cap = (long long)sm_count() * 8;              // 8 x 256 threads = 64 warps per SM
