@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define VC_B200_ABI_VERSION 7
+#define VC_B200_ABI_VERSION 8
 
 int vc_abi_version(void);
 const char* vc_last_error(void);
@@ -70,6 +70,13 @@ typedef struct vc_gemm_desc {
   float* gn_part; int32_t gn_sub;
   /* optional: multi-GPU layout switch fused into the epilogue (see vc_gemm_peer below); NULL = write `out` locally */
   const struct vc_gemm_peer* peer;
+  /* FP8 mode (new functionality, no reference counterpart): fp8 = 1 makes `w` e4m3 weights (ldw in elements) with per-output-channel
+   * scales w_scale[N]; A stays fp16 and is converted to e4m3 inside the kernel with s_a = *a_amax / 448 (1 if *a_amax == 0),
+   * a_amax being a device scalar written by vc_absmax_f16 over everything the GEMM reads.  The epilogue starts from
+   * acc * (s_a * w_scale[n]).  Needs K % 16 == 0; no out_f32, no peer.  A zero-initialised tail keeps the fp16 GEMM. */
+  int32_t fp8;
+  const float* w_scale;
+  const float* a_amax;
 } vc_gemm_desc;
 /* Output rows of the GEMM are stored tile by tile (TMA stores through the NVLink peer mapping) into the receive buffers of the ranks
  * that own them in the OTHER layout of the frame-sharded U-Net (SURVEY.md 8e; new functionality): mode 1 = this rank's rows are
@@ -83,6 +90,10 @@ typedef struct vc_gemm_peer {
 int vc_gemm_tap(const vc_gemm_desc* d, void* stream);
 /* N-tile width the kernel will use for (N, geglu): needed to interleave GEGLU weights on the host */
 int vc_gemm_tile_n(int32_t N, int32_t geglu);
+/* *amax = max |x| over `rows` rows of [x1 (cols1 columns, row pitch ld1) | x2 (cols2, pitch ld2; NULL if unused)], fp32: the
+ * per-tensor activation scale of an FP8 vc_gemm_tap.  Columns and pitches multiples of 8, rows 16-byte aligned. */
+int vc_absmax_f16(const void* x1, int64_t rows, int32_t cols1, int32_t ld1, const void* x2, int32_t cols2, int32_t ld2, float* amax,
+                  void* stream);
 
 /* ---- fused attention, head_dim 64 ---------------------------------------------------------------------------
  * replaces: CrossAttention.forward / efficient_forward, lvdm/modules/attention.py:81-144 / 146-209

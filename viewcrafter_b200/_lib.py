@@ -10,7 +10,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("VC_B200_LIB") or os.path.join(_HERE, "libvc_b200.so")   # override: A/B builds of the kernels
 
-ABI_VERSION = 7
+ABI_VERSION = 8
 
 
 class VcError(RuntimeError):
@@ -26,7 +26,7 @@ class GemmDesc(C.Structure):
                 ("bias", C.c_void_p), ("bias_z_div", C.c_int32), ("res", C.c_void_p), ("ldr", C.c_int32),
                 ("geglu", C.c_int32), ("ln_stats", C.c_void_p), ("ln_colsum", C.c_void_p), ("ln_part", C.c_void_p),
                 ("ldo_y", C.c_int64), ("ldo_z", C.c_int64), ("gn_part", C.c_void_p), ("gn_sub", C.c_int32),
-                ("peer", C.c_void_p)]
+                ("peer", C.c_void_p), ("fp8", C.c_int32), ("w_scale", C.c_void_p), ("a_amax", C.c_void_p)]
 
 
 class GemmPeer(C.Structure):
@@ -68,6 +68,7 @@ SIGNATURES = {
     "vc_reset_launch_count": (None, []),
     "vc_gemm_tap": (C.c_int, [C.POINTER(GemmDesc), _vp]),
     "vc_gemm_tile_n": (C.c_int, [_i32, _i32]),
+    "vc_absmax_f16": (C.c_int, [_vp, _i64, _i32, _i32, _vp, _i32, _i32, _vp, _vp]),
     "vc_flash_attn_d64": (C.c_int, [C.POINTER(AttnDesc), _vp]),
     "vc_temporal_attn": (C.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _i32, _i64, _i32, _f32, _vp]),
     "vc_groupnorm_ws_bytes": (_sz, [_i32]),

@@ -35,6 +35,7 @@ int vc_gemm_tap(const vc_gemm_desc* c, void* stream) {
   d.bias = c->bias; d.bias_z_div = c->bias_z_div; d.res = H(c->res); d.ldr = c->ldr; d.geglu = c->geglu;
   d.ln_stats = c->ln_stats; d.ln_colsum = c->ln_colsum; d.ln_part = c->ln_part; d.gn_part = c->gn_part; d.gn_sub = c->gn_sub;
   d.ldo_y = c->ldo_y; d.ldo_z = c->ldo_z;
+  d.fp8 = c->fp8; d.w_scale = c->w_scale; d.a_amax = c->a_amax;
   GemmPeerDesc pd;
   if (c->peer && c->peer->mode) {
     const vc_gemm_peer* q = c->peer;
@@ -48,6 +49,11 @@ int vc_gemm_tap(const vc_gemm_desc* c, void* stream) {
   return gemm_tap(d, ST(stream));
 }
 int vc_gemm_tile_n(int32_t N, int32_t geglu) { return vc::pick_bn_public(N, geglu); }
+int vc_absmax_f16(const void* x1, int64_t rows, int32_t cols1, int32_t ld1, const void* x2, int32_t cols2, int32_t ld2, float* amax,
+                  void* stream) {
+  COUNT(1);
+  return absmax_f16(H(x1), rows, cols1, ld1, H(x2), cols2, ld2, amax, ST(stream));
+}
 
 int vc_flash_attn_d64(const vc_attn_desc* c, void* stream) {
   if (!c) { set_error("vc_flash_attn_d64: null descriptor"); return VC_ERR_ARG; }

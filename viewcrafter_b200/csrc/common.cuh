@@ -37,9 +37,10 @@ const char* last_error();
   } while (0)
 
 // Encode a tiled fp16 tensor map (rank 2..5), zero OOB fill; swizzle_bytes: 128 (default), 64 or 0 (none).
-// dims/box: innermost first.  strides_bytes: for dims 1..rank-1.
+// dims/box: innermost first, in elements.  strides_bytes: for dims 1..rank-1.  dtype: UINT8 for e4m3 weights.
 int encode_tmap_f16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
-                    const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes = 128);
+                    const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes = 128,
+                    CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
 
 int sm_count();   // of the CURRENT device (cached per device)
 
@@ -168,6 +169,17 @@ __device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr, uint32_
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
   d |= (uint64_t)1 << 62;   // SWIZZLE_128B
+  return d;
+}
+
+// The same for K-major e4m3 tiles of 64-byte rows (64 fp8), as TMA writes them with CU_TENSOR_MAP_SWIZZLE_64B: SBO = 512 B
+// between 8-row groups; one k32 step is 32 bytes along the row (tiles 512-byte aligned).
+__device__ __forceinline__ uint64_t wgmma_desc_sw64(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(512 >> 4) << 32;
+  d |= (uint64_t)2 << 62;   // SWIZZLE_64B
   return d;
 }
 

@@ -101,6 +101,10 @@ struct GemmParams {
   int vec_ok;            // output rows are 32-byte aligned: whole 32-column chunks of a non-TMA output are stored as 256-bit vectors
   int res_vec;           // residual rows are 32-byte aligned: whole 32-column chunks of the residual are loaded as 256-bit vectors
   GemmPeer peer;         // output scattered to the ranks of the frame group (mode != 0: `out` itself is not written)
+  // FP8 mode (gemm_tap_kernel<BN, true>): e4m3 weights, A converted to e4m3 in registers with the per-tensor scale
+  // s_a = a_amax / 448; the epilogue starts from acc * (s_a * w_scale[n])
+  const float* w_scale;  // [N] per-output-channel weight scales
+  const float* a_amax;   // device scalar: max |A| over everything the GEMM reads (absmax_f16)
 };
 
 struct TileCoord {
@@ -328,13 +332,31 @@ __device__ __forceinline__ void gn_part_accumulate(const GemmParams& p, const Ep
   }
 }
 
+// FP8 dequantisation of one 32-column chunk: f = acc * (s_a * w_scale[n]), in fp32
+__device__ __forceinline__ void fp8_dequant32(const GemmParams& p, int nb, float sa, float (&f)[32]) {
+  if (nb + 32 <= p.N) {
+#pragma unroll
+    for (int e = 0; e < 32; e += 4) {
+      const float4 w4 = __ldg(reinterpret_cast<const float4*>(p.w_scale + nb + e));
+      f[e] *= sa * w4.x; f[e + 1] *= sa * w4.y; f[e + 2] *= sa * w4.z; f[e + 3] *= sa * w4.w;
+    }
+  } else {
+#pragma unroll
+    for (int e = 0; e < 32; ++e)
+      if (nb + e < p.N) f[e] *= sa * __ldg(p.w_scale + nb + e);
+  }
+}
+
 // One 32-column chunk of this thread's row: folded LayerNorm, bias, residual, output statistics, store.
 // nb: first column in the accumulator's N space (bias / LayerNorm column sums / residual / statistics), col0: first output column.
 // plain: the values are final already (GEGLU, computed on the fragments), only statistics-free storing remains.
 // The residual is added here, in registers, whatever the store path: the statistics and every store path see the same values.
+// FP8: f holds the raw e4m3 products' sums; they are dequantised with the activation scale sa first, then the fp16 epilogue runs.
+template <bool FP8 = false>
 __device__ __forceinline__ void epi_chunk(const GemmParams& p, const EpiTile& t, int nb, int col0, int n_out, bool plain, float (&f)[32],
-                                          uint8_t* stage, int lane) {
+                                          uint8_t* stage, int lane, float sa = 1.f) {
   if (!plain) {
+    if constexpr (FP8) fp8_dequant32(p, nb, sa, f);
     if (p.ln_stats) {                              // folded LayerNorm (host guarantees N % 32 == 0)
       const float2 ln = t.row_ok ? __ldg(reinterpret_cast<const float2*>(p.ln_stats) + t.orow) : make_float2(0.f, 1.f);
 #pragma unroll

@@ -21,16 +21,24 @@
 //   next tile's stages only once the other one has seen all of its own.  Besides keeping the two mainloops from sharing the
 //   tensor cores, this keeps every full-barrier wait within one phase of the barrier, which the parity waits require.
 // Tiles are ordered n-fastest so CTAs that run concurrently share A tiles in L2.
+//
+// FP8 variant (FP8 = true, GemmDesc::fp8): the weights are e4m3 (per-output-channel scales w_scale), a ring stage holds
+// the fp16 A tile as before and the weight tile as 64-byte rows (64B swizzle).  The MMA warpgroup reads its A fragments from
+// the fp16 stage, scales them by 1 / s_a (s_a = a_amax / 448, one scale per GEMM call) and converts them to e4m3 in
+// registers (round to nearest, saturating), then issues wgmma m64nBNk32 e4m3 x e4m3 with A from registers.  A stays fp16 in
+// HBM: no conversion pass.  The epilogue starts from acc * (s_a * w_scale[n]) and is otherwise the fp16 one.
+#include <cuda_fp8.h>
+
 #include "gemm_common.cuh"
 #include "kernels.h"
 #include "wgmma.cuh"
 
 namespace vc {
 
-template <int BN>
+template <int BN, bool FP8 = false>
 struct GemmCfg {
   static constexpr int A_BYTES = BM * BK * 2;
-  static constexpr int B_BYTES = BN * BK * 2;
+  static constexpr int B_BYTES = BN * BK * (FP8 ? 1 : 2);
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int BUDGET = 227 * 1024 - 1024 /*align slack*/ - 256 /*barriers*/ - EPI_SMEM_BYTES;
   static constexpr int STAGES = BUDGET / STAGE_BYTES > 8 ? 8 : BUDGET / STAGE_BYTES;
@@ -42,9 +50,9 @@ struct GemmCfg {
 // Drain the accumulator fragments of one 64-row half of an MMA warpgroup's tile (64 rows x NCOLS columns) through the
 // warpgroup's transpose buffer, 64 columns at a time, and run the per-chunk epilogue with one row per thread: warp wl of the
 // warpgroup takes rows (wl & 1) * 32 + lane of the half and chunk (wl >> 1) of each 64-column slab.
-template <int BN, int NCOLS>
+template <int BN, int NCOLS, bool FP8 = false>
 __device__ __forceinline__ void epi_drain(const GemmParams& p, const EpiTile& t, float (&acc)[BN / 2], float* xpose, int cw, int wl, int lane,
-                                          uint8_t* stage, bool plain, int nb0, int col0, int n_out) {
+                                          uint8_t* stage, bool plain, int nb0, int col0, int n_out, float sa = 1.f) {
   constexpr int SLABS = (NCOLS + 63) / 64;
   const int fr = 16 * wl + (lane >> 2), fc = 2 * (lane & 3);   // fragment row / column of d[j * 4] (wgmma accumulator layout)
 #pragma unroll
@@ -69,14 +77,26 @@ __device__ __forceinline__ void epi_drain(const GemmParams& p, const EpiTile& t,
         const float4 v = src[e];
         f[4 * e] = v.x; f[4 * e + 1] = v.y; f[4 * e + 2] = v.z; f[4 * e + 3] = v.w;
       }
-      epi_chunk(p, t, nb0 + c * 32, col0 + c * 32, n_out, plain, f, stage, lane);
+      epi_chunk<FP8>(p, t, nb0 + c * 32, col0 + c * 32, n_out, plain, f, stage, lane, sa);
     }
   }
 }
 
-template <int BN>
+// e4m3 A fragment register of wgmma k32: 4 consecutive fp16 of one row (8 bytes of the 128B-swizzled stage), each scaled by
+// inv_sa in fp32 and rounded once to e4m3 (satfinite); element k in byte k
+__device__ __forceinline__ uint32_t a_frag_e4m3(uint32_t addr, float inv_sa) {
+  uint32_t u0, u1;
+  asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(u0), "=r"(u1) : "r"(addr));
+  const float2 lo = __half22float2(*reinterpret_cast<const __half2*>(&u0));
+  const float2 hi = __half22float2(*reinterpret_cast<const __half2*>(&u1));
+  const uint32_t q0 = __nv_cvt_float2_to_fp8x2(make_float2(lo.x * inv_sa, lo.y * inv_sa), __NV_SATFINITE, __NV_E4M3);
+  const uint32_t q1 = __nv_cvt_float2_to_fp8x2(make_float2(hi.x * inv_sa, hi.y * inv_sa), __NV_SATFINITE, __NV_E4M3);
+  return q0 | (q1 << 16);
+}
+
+template <int BN, bool FP8>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tap_kernel(const __grid_constant__ GemmParams p) {
-  using Cfg = GemmCfg<BN>;
+  using Cfg = GemmCfg<BN, FP8>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -142,6 +162,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tap_kernel(const __grid_
     uint8_t* stage = epi_smem + (warp - 4) * EPI_STAGE_BYTES;
     float* xpose = reinterpret_cast<float*>(epi_smem + EPI_WARPS * EPI_STAGE_BYTES + cw * EPI_XPOSE_BYTES);
     const uint32_t ring = smem_u32(smem);
+    float sa = 1.f, inv_sa = 1.f;                   // FP8: per-tensor activation scale s_a = amax / 448 (1 for an all-zero A)
+    if constexpr (FP8) {
+      const float amax = *p.a_amax;
+      sa = amax > 0.f ? __fdiv_rn(amax, 448.f) : 1.f;
+      inv_sa = __fdiv_rn(1.f, sa);
+    }
     float acc[2][BN / 2];                           // rows [0, 64) and [64, 128) of the tile
 #pragma unroll
     for (int h = 0; h < 2; ++h)
@@ -164,18 +190,49 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tap_kernel(const __grid_
         mbar_wait(&full_bar[s], ph);
         const uint32_t a_addr = ring + s * Cfg::STAGE_BYTES;
         const uint32_t b_addr = ring + s * Cfg::STAGE_BYTES + Cfg::A_BYTES;
-        wgmma_fence();
+        if constexpr (!FP8) {
+          wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-          const uint64_t db = wgmma_desc_sw128(b_addr + 32 * k);
-          Wgmma<BN>::ss(acc[0], wgmma_desc_sw128(a_addr + 32 * k), db, (i > 0 || k > 0) ? 1 : 0);
-          Wgmma<BN>::ss(acc[1], wgmma_desc_sw128(a_addr + 64 * BK * 2 + 32 * k), db, (i > 0 || k > 0) ? 1 : 0);
-        }
-        wgmma_commit();
-        wgmma_wait<1>();                            // the previous k-block's MMAs have retired: its stage may be refilled
-        if (prev >= 0) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&empty_bar[prev]);
+          for (int k = 0; k < BK / 16; ++k) {
+            const uint64_t db = wgmma_desc_sw128(b_addr + 32 * k);
+            Wgmma<BN>::ss(acc[0], wgmma_desc_sw128(a_addr + 32 * k), db, (i > 0 || k > 0) ? 1 : 0);
+            Wgmma<BN>::ss(acc[1], wgmma_desc_sw128(a_addr + 64 * BK * 2 + 32 * k), db, (i > 0 || k > 0) ? 1 : 0);
+          }
+          wgmma_commit();
+          wgmma_wait<1>();                            // the previous k-block's MMAs have retired: its stage may be refilled
+          if (prev >= 0) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[prev]);
+          }
+        } else {
+          // A fragment of wgmma k32 (8-bit): register j of thread (g = lane / 4, q = lane % 4) holds row g + 8 (j & 1) of the
+          // warp's 16 rows, k = 16 (j >> 1) + 4 q .. + 3.  In the 128B-swizzled fp16 stage that is 16-byte chunk
+          // c = 4 ks + 2 (j >> 1) + q / 2 of the row, stored at chunk c ^ (row & 7) = c ^ g, byte 8 (q & 1) inside it.
+          // One commit group per k32 step: the conversion of the next step overlaps the MMAs of this one, and only two steps'
+          // fragments (16 registers) are live at a time.
+          const int g = lane >> 2, q = lane & 3;
+          const uint32_t a_row = a_addr + (16 * wl + g) * (BK * 2) + (q & 1) * 8;
+#pragma unroll
+          for (int ks = 0; ks < BK / 32; ++ks) {
+            const uint64_t db = wgmma_desc_sw64(b_addr + 32 * ks);
+            uint32_t fa[2][4];
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                const int c = 4 * ks + 2 * (j >> 1) + (q >> 1);
+                fa[h][j] = a_frag_e4m3(a_row + (h * 64 + 8 * (j & 1)) * (BK * 2) + ((c ^ g) << 4), inv_sa);
+              }
+            wgmma_fence();
+            WgmmaF8<BN>::rs(acc[0], fa[0], db, (i > 0 || ks > 0) ? 1 : 0);
+            WgmmaF8<BN>::rs(acc[1], fa[1], db, (i > 0 || ks > 0) ? 1 : 0);
+            wgmma_commit();
+            wgmma_wait<1>();                          // ks = 0: the previous k-block's last step has retired
+            if (ks == 0 && prev >= 0) {
+              __syncwarp();
+              if (lane == 0) mbar_arrive(&empty_bar[prev]);
+            }
+          }
         }
         prev = s;
         if (++s == STAGES) { s = 0; ph ^= 1; }
@@ -194,7 +251,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tap_kernel(const __grid_
         const EpiTile t = epi_tile(p, tile, h * 2 + (wl & 1), lane);
         const int n0 = t.n_tile * BN;
         if (BN != 128 || !p.geglu) {                   // GEGLU always runs at BN = 128 (pick_bn)
-          epi_drain<BN, BN>(p, t, acc[h], xpose, cw, wl, lane, stage, false, n0, n0, p.N);
+          epi_drain<BN, BN, FP8>(p, t, acc[h], xpose, cw, wl, lane, stage, false, n0, n0, p.N, sa);
         } else {
           // GEGLU on the fragments: tile columns [0, BN/2) are values, [BN/2, BN) the matching gates (weights were interleaved
           // per tile); out[:, n_tile*BN/2 + c] = (value + bias_v) * gelu(gate + bias_g).  No residual (checked on the host).
@@ -216,6 +273,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tap_kernel(const __grid_
             for (int e = 0; e < 4; ++e) {
               const int n = n0 + 8 * j + 2 * (lane & 3) + (e & 1);
               float a = acc[h][j * 4 + e], g = acc[h][(j + HALF / 8) * 4 + e];
+              if constexpr (FP8) {
+                a *= sa * __ldg(p.w_scale + n);
+                g *= sa * __ldg(p.w_scale + n + HALF);
+              }
               if (p.ln_stats) {
                 const float2 l = ln[e >> 1];
                 a = (a - l.x * __ldg(p.ln_colsum + n)) * l.y;
@@ -233,25 +294,27 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tap_kernel(const __grid_
   }
 }
 
-template <int BN>
+template <int BN, bool FP8 = false>
 static int launch_gemm(const GemmParams& p, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN>;
+  using Cfg = GemmCfg<BN, FP8>;
   static DeviceOnce configured;
   if (device_once_needed(configured)) {
-    VC_CHECK_CUDA(cudaFuncSetAttribute(gemm_tap_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    VC_CHECK_CUDA(cudaFuncSetAttribute(gemm_tap_kernel<BN, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     device_once_mark(configured);
   }
   const int grid = p.total_tiles < sm_count() ? p.total_tiles : sm_count();
-  gemm_tap_kernel<BN><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(p);
+  gemm_tap_kernel<BN, FP8><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(p);
   VC_CHECK_CUDA(cudaGetLastError());
   return VC_OK;
 }
 
 // Widest tile that divides N: the accumulator lives in registers (BN / 2 per MMA thread), so tiles stop at 160 columns.
-static int pick_bn(int N, int geglu) {
+// FP8 stops at 128: its A fragments take the registers that 160 columns would need (ptxas spills), so N = 320 runs at 64.
+static int pick_bn(int N, int geglu, int fp8 = 0) {
   if (geglu) return 128;
   if (N <= 32) return 32;
   if (N <= 64) return 64;
+  if (fp8 && N % 160 == 0) return N % 128 == 0 ? 128 : 64;
   if (N % 160 == 0) return 160;
   if (N % 128 == 0) return 128;
   if (N % 96 == 0 && N <= 192) return 96;
@@ -277,12 +340,19 @@ int gemm_tap(const GemmDesc& d, cudaStream_t stream) {
   VC_REQUIRE(!d.bias || (reinterpret_cast<uintptr_t>(d.bias) & 15) == 0, "gemm_tap: bias must be 16-byte aligned");
   VC_REQUIRE(!d.bias || d.bias_z_div <= 0 || d.N % 4 == 0, "gemm_tap: per-z bias rows (bias_z_div=%d) need N %% 4 == 0 (N=%d)",
              d.bias_z_div, d.N);
+  if (d.fp8) {
+    VC_REQUIRE(d.K % 16 == 0, "gemm_tap: fp8 needs K %% 16 == 0 (K=%d)", d.K);
+    VC_REQUIRE(d.w_scale && d.a_amax, "gemm_tap: fp8 needs w_scale and a_amax");
+    VC_REQUIRE((reinterpret_cast<uintptr_t>(d.w_scale) & 15) == 0, "gemm_tap: fp8 w_scale must be 16-byte aligned");
+    VC_REQUIRE(!d.out_f32, "gemm_tap: fp8 does not support an fp32 output");
+    VC_REQUIRE(!(d.peer && d.peer->mode), "gemm_tap: fp8 does not support the peer-scatter epilogue");
+  }
   const void* optr = d.out_f32 ? (const void*)d.out_f32 : (const void*)d.out;
   const int esz = d.out_f32 ? 4 : 2;
 
   GemmParams p;
   memset(&p, 0, sizeof(p));
-  const int BN = pick_bn(d.N, d.geglu);
+  const int BN = pick_bn(d.N, d.geglu, d.fp8);
   p.bx = d.bx; p.by = d.by; p.X = d.X; p.Y = d.Y; p.Z = d.Z;
   p.tiles_x = (d.X + d.bx - 1) / d.bx;
   p.tiles_y = (d.Y + d.by - 1) / d.by;
@@ -313,9 +383,11 @@ int gemm_tap(const GemmDesc& d, cudaStream_t stream) {
   }
   {
     uint64_t dims[2] = {(uint64_t)d.K, (uint64_t)d.num_taps * d.N};
-    uint64_t str[1] = {(uint64_t)(d.ldw > 0 ? d.ldw : d.K) * 2};
+    const int wbytes = d.fp8 ? 1 : 2;
+    uint64_t str[1] = {(uint64_t)(d.ldw > 0 ? d.ldw : d.K) * wbytes};
     uint32_t box[2] = {(uint32_t)BK, (uint32_t)BN};
-    int rc = encode_tmap_f16(&p.tmap_b, d.w, 2, dims, str, box);
+    int rc = d.fp8 ? encode_tmap_f16(&p.tmap_b, d.w, 2, dims, str, box, 64, CU_TENSOR_MAP_DATA_TYPE_UINT8)
+                   : encode_tmap_f16(&p.tmap_b, d.w, 2, dims, str, box);
     if (rc) return rc;
   }
   p.N = d.N; p.K = d.K; p.K1 = d.K1;
@@ -325,6 +397,7 @@ int gemm_tap(const GemmDesc& d, cudaStream_t stream) {
   p.bias = d.bias; p.bias_z_div = d.bias_z_div;
   p.res = d.res; p.ldr = d.ldr;
   p.geglu = d.geglu;
+  p.w_scale = d.w_scale; p.a_amax = d.a_amax;
   VC_REQUIRE((d.ln_stats == nullptr) == (d.ln_colsum == nullptr), "gemm_tap: ln_stats and ln_colsum go together");
   VC_REQUIRE(!d.ln_stats || (d.num_taps == 1 && d.N % 32 == 0 && d.Y == 1 && d.Z == 1 && !d.a2),
              "gemm_tap: folded LayerNorm needs a plain [M,K] x [N,K] GEMM with N %% 32 == 0");
@@ -397,6 +470,14 @@ int gemm_tap(const GemmDesc& d, cudaStream_t stream) {
   const long long total = m_tiles * p.n_tiles;
   VC_REQUIRE(total > 0 && total < (1ll << 31), "gemm_tap: tile count %lld out of range", total);
   p.total_tiles = (int)total;
+  if (d.fp8) {
+    switch (BN) {
+      case 32: return launch_gemm<32, true>(p, stream);
+      case 64: return launch_gemm<64, true>(p, stream);
+      case 96: return launch_gemm<96, true>(p, stream);
+      case 128: return launch_gemm<128, true>(p, stream);
+    }
+  }
   switch (BN) {
     case 32: return launch_gemm<32>(p, stream);
     case 64: return launch_gemm<64>(p, stream);

@@ -68,7 +68,7 @@ static EncodeTiledFn get_encode() {
 }
 
 int encode_tmap_f16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                    const uint32_t* box, int swizzle_bytes) {
+                    const uint32_t* box, int swizzle_bytes, CUtensorMapDataType dtype) {
   EncodeTiledFn fn = get_encode();
   if (!fn) {
     set_error("cuTensorMapEncodeTiled is unavailable (no CUDA driver?)");
@@ -93,7 +93,7 @@ int encode_tmap_f16(CUtensorMap* out, const void* base, int rank, const uint64_t
     set_error("tensor map base address is not 16-byte aligned");
     return VC_ERR_ARG;
   }
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bdim, estr,
+  CUresult r = fn(out, dtype, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bdim, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_NONE,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {

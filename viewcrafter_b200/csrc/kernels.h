@@ -49,8 +49,15 @@ struct GemmDesc {
   float* gn_part = nullptr;
   int gn_sub = 0;
   const GemmPeerDesc* peer = nullptr;
+  // FP8 mode: w points to e4m3 weights (ldw in elements = bytes), out[r, n] starts from acc * (s_a * w_scale[n]) with
+  // s_a = *a_amax / 448 (1 if 0); A is converted to e4m3 in the kernel.  K % 16 == 0, no fp32 output, no peer scatter.
+  int fp8 = 0;
+  const float* w_scale = nullptr;
+  const float* a_amax = nullptr;
 };
 int gemm_tap(const GemmDesc& d, cudaStream_t stream);
+// *amax = max |x| over rows x [x1 (cols1 columns, pitch ld1) | x2 (cols2, pitch ld2)]: the FP8 GEMM's per-tensor activation scale
+int absmax_f16(const __half* x1, long long rows, int cols1, int ld1, const __half* x2, int cols2, int ld2, float* amax, cudaStream_t stream);
 
 struct AttnDesc {
   // q [B, Nq, heads, 64] (row pitch ldq), k/v [Bk, Nk, heads, 64] (pitch ldk/ldv), out [B, Nq, heads*64] (pitch ldo).

@@ -54,6 +54,51 @@ int im2col3x3_s2_nhwc(const __half* x, __half* out, int N, int H, int W, int C, 
 }
 
 // ------------------------------------------------------------------------------------------------
+// max |x| of one or two fp16 row blocks (the FP8 GEMM's activation scale).  Max is exact and order-independent, so the result
+// does not depend on the launch: every CTA folds its 8-element vectors with __hmax2, then one atomicMax on the float bits
+// (non-negative floats order like their bit patterns) into *amax, which the host zeroes first in stream order.
+// ------------------------------------------------------------------------------------------------
+__global__ void absmax_kernel(const __half* __restrict__ x1, int vec1, int ld1, const __half* __restrict__ x2, int vec2, int ld2,
+                              long long rows, unsigned int* __restrict__ amax) {
+  const unsigned vecs = vec1 + vec2;
+  const unsigned total = (unsigned)(rows * vecs);       // < 2^31 (host check): 32-bit index arithmetic
+  __half2 m = __float2half2_rn(0.f);
+  for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+    const unsigned r = i / vecs;
+    const int v = (int)(i - r * vecs);
+    const uint4 u = v < vec1 ? __ldg(reinterpret_cast<const uint4*>(x1 + (long long)r * ld1 + v * 8))
+                             : __ldg(reinterpret_cast<const uint4*>(x2 + (long long)r * ld2 + (v - vec1) * 8));
+    const __half2* h = reinterpret_cast<const __half2*>(&u);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) m = __hmax2(m, __habs2(h[e]));
+  }
+  float f = fmaxf(__low2float(m), __high2float(m));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) f = fmaxf(f, __shfl_xor_sync(0xffffffffu, f, o));
+  __shared__ float wmax[32];
+  if ((threadIdx.x & 31) == 0) wmax[threadIdx.x >> 5] = f;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < (int)(blockDim.x >> 5); ++w) f = fmaxf(f, wmax[w]);
+    atomicMax(amax, __float_as_uint(f));
+  }
+}
+int absmax_f16(const __half* x1, long long rows, int cols1, int ld1, const __half* x2, int cols2, int ld2, float* amax, cudaStream_t stream) {
+  VC_REQUIRE(x1 && amax && rows > 0 && cols1 > 0 && (!x2 || cols2 > 0), "absmax_f16: bad arguments");
+  VC_REQUIRE(cols1 % 8 == 0 && ld1 % 8 == 0 && (reinterpret_cast<uintptr_t>(x1) & 15) == 0 &&
+                 (!x2 || (cols2 % 8 == 0 && ld2 % 8 == 0 && (reinterpret_cast<uintptr_t>(x2) & 15) == 0)),
+             "absmax_f16: rows must be 16-byte aligned with a multiple of 8 columns");
+  const int vec2 = x2 ? cols2 / 8 : 0;
+  const long long total = rows * (cols1 / 8 + vec2);
+  VC_REQUIRE(total < (1ll << 31), "absmax_f16: %lld vectors out of range", total);
+  const int blocks = (int)min((long long)sm_count() * 4, (total + 255) / 256);
+  VC_CHECK_CUDA(cudaMemsetAsync(amax, 0, sizeof(float), stream));
+  absmax_kernel<<<blocks, 256, 0, stream>>>(x1, cols1 / 8, ld1, x2, vec2, ld2, rows, reinterpret_cast<unsigned int*>(amax));
+  VC_CHECK_CUDA(cudaGetLastError());
+  return VC_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
 // layout conversions at the boundary ([B,C,T,H,W] fp32 <-> [(B T) H W, C] fp16/fp32)
 // ------------------------------------------------------------------------------------------------
 __global__ void nchw_to_nhwc_kernel(const float* __restrict__ x, __half* __restrict__ out, int B, int C, int T, long long HW,

@@ -137,6 +137,69 @@ def pack_geglu_ln(w: torch.Tensor, b: torch.Tensor, gamma: torch.Tensor, beta: t
     return w16[idx].contiguous(), b2[idx].contiguous(), cs[idx].contiguous()
 
 
+FP8_MAX = 448.0     # largest finite e4m3 value
+
+
+class Fp8Weight:
+    """A packed GEMM weight in FP8 mode: e4m3 values ``q`` [taps * N, K] (torch.float8_e4m3fn) and per-output-channel fp32 scales
+    ``scale`` [N]; the weight the GEMM multiplies is q * scale[n].  Built by pack_fp8; every tap-GEMM wrapper accepts it for ``w``."""
+    __slots__ = ("q", "scale")
+
+    def __init__(self, q: torch.Tensor, scale: torch.Tensor):
+        self.q, self.scale = q, scale
+
+    @property
+    def shape(self):
+        return self.q.shape
+
+    def dequant(self) -> torch.Tensor:
+        """fp32 [taps * N, K]: the weights the FP8 GEMM multiplies."""
+        taps = self.q.shape[0] // self.scale.shape[0]
+        return (self.q.float().view(taps, -1, self.q.shape[1]) * self.scale[None, :, None]).view(self.q.shape)
+
+
+def pack_fp8(w_packed: torch.Tensor, taps: int = 1):
+    """Quantise an already packed fp16 GEMM weight [taps * N, K] (rows tap * N + n) to e4m3 per output channel n:
+    s_w[n] = max over taps and k of |w[n]| / 448 (1 for an all-zero channel), q_w = e4m3_rn(w / s_w[n]) (clamped to +-448).
+    Returns (q_w as torch.float8_e4m3fn, s_w fp32 [N])."""
+    rows, K = w_packed.shape
+    assert rows % taps == 0
+    w = w_packed.detach().float().view(taps, rows // taps, K)
+    amax = w.abs().amax(dim=(0, 2))
+    s = torch.where(amax > 0, amax / FP8_MAX, torch.ones_like(amax))
+    q = (w / s[None, :, None]).clamp(-FP8_MAX, FP8_MAX).to(torch.float8_e4m3fn)
+    return q.view(rows, K).contiguous(), s.contiguous()
+
+
+def fp8_colsum(w8: Fp8Weight) -> torch.Tensor:
+    """ln_colsum of a LayerNorm-folded FP8 weight: the column sums of the DEQUANTISED weights, which the GEMM multiplies."""
+    return w8.dequant().sum(1).contiguous()
+
+
+def absmax(x: torch.Tensor, x2: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """fp32 [1] device scalar max |[x | x2]| over every row: the per-tensor activation scale of the FP8 GEMM (s_a = amax / 448)."""
+    _chk16(x, "absmax.x")
+    if x2 is not None:
+        _chk16(x2, "absmax.x2")
+        assert x2.shape[0] == x.shape[0]
+    if out is None:
+        out = torch.empty(1, device=x.device, dtype=torch.float32)
+    check(_lib.load().vc_absmax_f16(x.data_ptr(), x.shape[0], x.shape[1], x.stride(0), _ptr(x2), 0 if x2 is None else x2.shape[1],
+                                    0 if x2 is None else x2.stride(0), out.data_ptr(), _stream()), "vc_absmax_f16")
+    return out
+
+
+def _set_w(d: GemmDesc, w, amax: Optional[torch.Tensor]):
+    """Point the descriptor at the weight: fp16 [rows, K], or an Fp8Weight with the activation's absmax scalar."""
+    if isinstance(w, Fp8Weight):
+        assert amax is not None and w.q.is_cuda and w.q.dtype == torch.float8_e4m3fn
+        d.w, d.ldw = w.q.data_ptr(), w.q.stride(0)
+        d.fp8, d.w_scale, d.a_amax = 1, w.scale.data_ptr(), amax.data_ptr()
+    else:
+        _chk16(w, "gemm.w")
+        d.w, d.ldw = w.data_ptr(), w.stride(0)
+
+
 # ----------------------------------------------------------------------------------------------------
 # tensor-core ops
 # ----------------------------------------------------------------------------------------------------
@@ -248,8 +311,12 @@ def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None
     epilogue leaves per-32-column partial sums of the rows it is writing and a tiny kernel finishes them, so y is not re-read.
     gn_out: y feeds a GroupNorm next: leave its partial sums (GnPart, attached to y as ``y._vc_gn``; see groupnorm()).
     peer: a parallel.PeerFrameComm.scatter_plan(): the epilogue stores y into the other ranks' receive buffers (multi-GPU layout switch
-    fused into the GEMM); returns the switched tensor."""
-    _chk16(x, "linear.x"); _chk16(w, "linear.w")
+    fused into the GEMM); returns the switched tensor.
+    w may be an Fp8Weight (FP8 mode): the absmax of [x|x2] is computed first and the GEMM runs e4m3 x e4m3."""
+    _chk16(x, "linear.x")
+    fp8 = isinstance(w, Fp8Weight)
+    if fp8 and peer is not None:
+        raise VcError("linear: FP8 weights do not support the multi-GPU peer-scatter epilogue")
     M, K1 = x.shape
     N, K = w.shape
     n_out = N // 2 if geglu else N
@@ -266,8 +333,8 @@ def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None
     else:
         assert K1 == K, (K1, K)
     d.X, d.Y, d.Z, d.bx, d.by = M, 1, 1, 128, 1
-    d.K, d.K1, d.w, d.N, d.num_taps = K, K1, w.data_ptr(), N, 1
-    d.ldw = w.stride(0)                                  # w may be a column slice of a wider matrix (e.g. K of a fused QK)
+    d.K, d.K1, d.N, d.num_taps = K, K1, N, 1
+    _set_w(d, w, absmax(x, x2) if fp8 else None)         # w may be a column slice of a wider matrix (e.g. K of a fused QK)
     if out_f32:
         d.out_f32 = out.data_ptr()
     else:
@@ -320,7 +387,10 @@ def conv3x3(x: torch.Tensor, frames: int, H: int, W: int, w9: torch.Tensor, bias
             res: Optional[torch.Tensor] = None, x2: Optional[torch.Tensor] = None, bias_z_div: int = 0,
             out_f32: bool = False, out: Optional[torch.Tensor] = None, gn_out: bool = False, peer=None) -> torch.Tensor:
     """3x3 / stride 1 / pad 1 convolution on [frames*H*W, Cin] rows; w9 = pack_conv3x3(weight).  gn_out / peer: see linear()."""
-    _chk16(x, "conv3x3.x"); _chk16(w9, "conv3x3.w")
+    _chk16(x, "conv3x3.x")
+    fp8 = isinstance(w9, Fp8Weight)
+    if fp8 and peer is not None:
+        raise VcError("conv3x3: FP8 weights do not support the multi-GPU peer-scatter epilogue")
     M, K1 = x.shape
     assert M == frames * H * W, (M, frames, H, W)
     K = w9.shape[1]
@@ -339,7 +409,8 @@ def conv3x3(x: torch.Tensor, frames: int, H: int, W: int, w9: torch.Tensor, bias
         assert K1 == K, (K1, K)
     d.X, d.Y, d.Z = W, H, frames
     d.bx, d.by = _conv_box(H, W)
-    d.K, d.K1, d.w, d.N, d.num_taps = K, K1, w9.data_ptr(), N, 9
+    d.K, d.K1, d.N, d.num_taps = K, K1, N, 9
+    _set_w(d, w9, absmax(x, x2) if fp8 else None)
     for t in range(9):
         d.tap_dx[t] = t % 3 - 1
         d.tap_dy[t] = t // 3 - 1
@@ -394,15 +465,16 @@ def upconv3x3(x: torch.Tensor, frames: int, H: int, W: int, packs, bias: Optiona
     N = packs[0].shape[0] // 4
     assert N % 32 == 0, "upconv3x3 writes through the TMA-store epilogue: Cout must be a multiple of 32"
     out = torch.empty((frames * 4 * H * W, N), device=x.device, dtype=torch.float16)
+    amax = absmax(x) if isinstance(packs[0], Fp8Weight) else None      # FP8: one activation scale for the four parities
     for a in (0, 1):
         for b in (0, 1):
             w4 = packs[a * 2 + b]
-            _chk16(w4, "upconv3x3.w")
             d = GemmDesc()
             d.a, d.lda = x.data_ptr(), x.stride(0)
             d.X, d.Y, d.Z = W, H, frames
             d.bx, d.by = _conv_box(H, W)
-            d.K, d.K1, d.w, d.N, d.num_taps = K, K, w4.data_ptr(), N, 4
+            d.K, d.K1, d.N, d.num_taps = K, K, N, 4
+            _set_w(d, w4, amax)
             for t in range(4):
                 d.tap_dx[t] = (t % 2) + b - 1
                 d.tap_dy[t] = (t // 2) + a - 1
@@ -417,6 +489,9 @@ def conv_temporal(x: torch.Tensor, B: int, T: int, HW: int, w3: torch.Tensor, bi
                   res: Optional[torch.Tensor] = None, gn_out: bool = False, peer=None) -> torch.Tensor:
     """Conv3d (3,1,1) pad (1,0,0) on [(B T) HW, C] rows: three row-shifted GEMM taps; batches never mix (Z = B).  gn_out: see linear()."""
     _chk16(x, "conv_temporal.x")
+    fp8 = isinstance(w3, Fp8Weight)
+    if fp8 and peer is not None:
+        raise VcError("conv_temporal: FP8 weights do not support the multi-GPU peer-scatter epilogue")
     M, K = x.shape
     assert M == B * T * HW
     N = w3.shape[0] // 3
@@ -426,7 +501,8 @@ def conv_temporal(x: torch.Tensor, B: int, T: int, HW: int, w3: torch.Tensor, bi
     d = GemmDesc()
     d.a, d.lda = x.data_ptr(), x.stride(0)
     d.X, d.Y, d.Z, d.bx, d.by = T * HW, 1, B, 128, 1
-    d.K, d.K1, d.w, d.N, d.num_taps = K, K, w3.data_ptr(), N, 3
+    d.K, d.K1, d.N, d.num_taps = K, K, N, 3
+    _set_w(d, w3, absmax(x) if fp8 else None)
     for t in range(3):
         d.tap_dx[t] = (t - 1) * HW
         d.tap_dy[t] = 0

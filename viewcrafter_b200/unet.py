@@ -41,6 +41,56 @@ def _ln_linear(Q: dict, x: torch.Tensor, name: str, ln: str, st=None, **kw) -> t
     return ops.linear(ops.layernorm(x, *Q[ln]), Q[name], bias=Q[name + "_b"], **kw)
 
 
+def _fp8(w, taps: int = 1) -> "ops.Fp8Weight":
+    return ops.Fp8Weight(*ops.pack_fp8(w, taps))
+
+
+# FP8 mode (UNetModel.enable_fp8): the packed weights each layer class runs in e4m3; everything else keeps its fp16 pack.
+# The first conv (K = 8 input channels), the last conv (N = 4 outputs) and the cached context K/V projections stay fp16.
+_FP8_RES = {"w1": 9, "w2": 9, "skip_w": 1}
+_FP8_TF = {"in_w": 1, "out_w": 1}
+_FP8_BLOCK = {"qkv1": 1, "o1_w": 1, "qkv2": 1, "q2": 1, "o2_w": 1, "ff1": 1, "ff2_w": 1}
+
+
+def _fp8_module(P: dict) -> dict:
+    """The FP8 counterpart of one packed block (a shallow copy sharing every fp16 tensor it keeps)."""
+    k, Q8 = P["kind"], dict(P)
+    if k == "R":
+        for name, taps in _FP8_RES.items():
+            if name in P:
+                Q8[name] = _fp8(P[name], taps)
+        if "tconv" in P:
+            Q8["tconv"] = [(g, b, _fp8(w3, 3), b3) for g, b, w3, b3 in P["tconv"]]
+    elif k in ("S", "T"):
+        for name, taps in _FP8_TF.items():
+            Q8[name] = _fp8(P[name], taps)
+        blocks = []
+        for Q in P["blocks"]:
+            B8 = dict(Q)
+            for name, taps in _FP8_BLOCK.items():
+                if name in Q:
+                    B8[name] = _fp8(Q[name], taps)
+                    if Q.get(name + "_cs") is not None:          # folded LayerNorm: column sums of the dequantised weights
+                        B8[name + "_cs"] = ops.fp8_colsum(B8[name])
+            blocks.append(B8)
+        Q8["blocks"] = blocks
+    elif k == "D":
+        Q8["w"] = _fp8(P["w"])
+    elif k == "U":
+        Q8["w"] = [_fp8(w, 4) for w in P["w"]] if isinstance(P["w"], list) else _fp8(P["w"], 9)
+    return Q8                                               # "C": the first conv stays fp16
+
+
+def _fp8_packs(P: dict) -> dict:
+    P8 = dict(P)
+    P8["input"] = [[_fp8_module(m) for m in stage] for stage in P["input"]]
+    if "init_attn" in P:
+        P8["init_attn"] = [_fp8_module(m) for m in P["init_attn"]]
+    P8["middle"] = [_fp8_module(m) for m in P["middle"]]
+    P8["output"] = [[_fp8_module(m) for m in stage] for stage in P["output"]]
+    return P8                                               # out_w (the last conv) stays fp16
+
+
 def _unsupported(flag: str):
     raise NotImplementedError(f"viewcrafter_b200.UNetModel: option {flag} is not on the ViewCrafter inference path")
 
@@ -222,13 +272,14 @@ class UNetModel(nn.Module):
         self._graph_mode = os.environ.get("VC_UNET_GRAPH", "0") == "1"     # see enable_cuda_graph
         self._graphs = {}
         self.graph_replayed_launches = 0    # kernels of this library executed through graph replays (bench.py's gpu_launches)
+        self._fp8, self._packed8 = False, None
         self.register_load_state_dict_post_hook(lambda module, incompatible: module.invalidate_packed())
 
     # ------------------------------------------------------------------------------------------
     # weight packing: fp32 checkpoint tensors -> kernel layouts (fp16 K-major GEMM operands, fp32 norm/bias)
     # ------------------------------------------------------------------------------------------
     def invalidate_packed(self):
-        self._packed = None
+        self._packed = self._packed8 = None
         self._kv_caches, self._kv_cache, self._canon = [], {}, []
         self._graphs = {}
 
@@ -244,11 +295,44 @@ class UNetModel(nn.Module):
             self._graphs = {}
         return self
 
+    def enable_fp8(self, on: bool = True):
+        """FP8 mode: every tap-GEMM of the forward except the first conv, the last conv and the cached context K/V projections
+        runs e4m3 x e4m3 with fp32 accumulation (weights per output channel, activations per tensor with a just-in-time absmax;
+        INTEGRATION.md "FP8 mode").  The e4m3 packs are built next to the fp16 ones; switching the mode off frees them and
+        returns exactly to the fp16 path.  Not batch-invariant, so it refuses reproducible mode; one GPU (or replica groups
+        of one GPU) only."""
+        if on:
+            if ops.reproducible():
+                raise ValueError("UNetModel.enable_fp8: FP8 mode is not batch-invariant (one activation scale per GEMM over the whole "
+                                 "batch) and cannot run in reproducible mode")
+            if self._comm is not None:
+                raise NotImplementedError("UNetModel.enable_fp8: FP8 mode runs on one GPU; this model is frame-sharded over several")
+        self._fp8 = bool(on)
+        if not on and self._packed8 is not None:
+            # the graphs captured in FP8 mode read the packs that go here
+            self._packed8 = None
+            self._graphs = {k: g for k, g in self._graphs.items() if not k[-2]}     # key[-2]: FP8 mode (_forward_graphed)
+        elif on and self.time_embed[0].weight.is_cuda:
+            self._packs()
+        return self
+
+    def fp8_enabled(self) -> bool:
+        return self._fp8
+
+    def _packs(self):
+        """The packed operands of the current mode (fp16, or the FP8 packs built from them)."""
+        P = self._packed or self._pack()
+        if not self._fp8:
+            return P
+        if self._packed8 is None:
+            self._packed8 = _fp8_packs(P)
+        return self._packed8
+
     def _apply(self, fn, *a, **k):
         # a pure device move (.cuda() / .to(device)) carries the packed kernel operands along (H2D copies, no repacking);
-        # anything that changes dtypes drops them
+        # anything that changes dtypes drops them.  The FP8 packs are rebuilt from the fp16 ones when next needed.
         packed = self._packed if ops.is_device_only(fn) else None
-        self._packed = None
+        self._packed = self._packed8 = None
         self._kv_caches, self._kv_cache, self._canon = [], {}, []
         self._graphs = {}
         r = super()._apply(fn, *a, **k)
@@ -534,7 +618,7 @@ class UNetModel(nn.Module):
         self._kv_cache = cache                     # most recent entry (introspection / tests)
 
         def project(Q, name, tokens, b):
-            k = (id(Q), name, b)
+            k = (id(Q[name]), name, b)          # the fp16 weight: the same tensor in the fp16 and the FP8 packs of a block
             if k not in cache:
                 cache[k] = ops.linear(tokens, Q[name])
             return cache[k]
@@ -556,7 +640,7 @@ class UNetModel(nn.Module):
     def _forward_graphed(self, x, timesteps, context, fs, kwargs):
         ver = ops.tensor_version(context)
         flags = tuple(sorted((k, bool(v)) for k, v in kwargs.items() if k == "cfg_shared_prefix"))
-        key = (tuple(x.shape), x.dtype, id(context), ver, fs is None, flags, id(self._comm), ops.reproducible())
+        key = (tuple(x.shape), x.dtype, id(context), ver, fs is None, flags, id(self._comm), self._fp8, ops.reproducible())
         e = self._graphs.get(key)
         if ver is None or (e is not None and e["ctx"] is not context):
             return self._forward_impl(x, timesteps, context, fs, kwargs)
@@ -592,7 +676,12 @@ class UNetModel(nn.Module):
 
     def _forward_impl(self, x, timesteps, context, fs, kwargs, gather=True):
         ops.require_cuda(x.device, "viewcrafter_b200.UNetModel")
-        P = self._packed or self._pack()
+        if self._fp8:
+            if ops.reproducible():
+                raise ValueError("UNetModel: FP8 mode cannot run in reproducible mode (enable_fp8(False) first)")
+            if self._comm is not None:
+                raise NotImplementedError("UNetModel: FP8 mode runs on one GPU; this model is frame-sharded over several")
+        P = self._packs()
         if P["device"] != x.device:
             raise ops.VcError(f"UNetModel weights are on {P['device']} but the input is on {x.device}")
         comm = self._comm
