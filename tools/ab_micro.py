@@ -16,7 +16,7 @@ def t(fn, reps=5):
     return e0.elapsed_time(e1) / reps * 1e-3
 
 
-tag = os.path.basename(_lib.LIB_PATH) + ("+bn64" if os.environ.get("VC_ATTN_BN64") == "1" else "") + ("+lnunroll" if os.environ.get("VC_LN_STATS_UNROLL") == "1" else "")
+tag = os.path.basename(_lib.LIB_PATH) + ("+bn64" if os.environ.get("VC_ATTN_BN64") == "1" else "")
 T = 25
 torch.manual_seed(0)
 for name, HW, heads in (("l0", 9216, 5), ("l1", 2304, 10), ("l2", 576, 20)):

@@ -198,7 +198,7 @@ static int bn64_mode() {
 }
 
 template <int BNK>
-static int launch_attn(const AttnDesc& d, cudaStream_t stream) {
+static int launch_attn(const vc_attn_desc& d, cudaStream_t stream) {
   using Cfg = AttnCfg<BNK>;
   AttnParams p;
   memset(&p, 0, sizeof(p));
@@ -220,7 +220,7 @@ static int launch_attn(const AttnDesc& d, cudaStream_t stream) {
     rc = encode_tmap_f16(&p.tmap_v, d.v, 4, dims, strv, box);
     if (rc) return rc;
   }
-  p.out = d.out; p.ldo = d.ldo; p.Nq = d.Nq; p.Nk = d.Nk; p.kv_shared = shared;
+  p.out = static_cast<__half*>(d.out); p.ldo = d.ldo; p.Nq = d.Nq; p.Nk = d.Nk; p.kv_shared = shared;
   p.scale_log2 = d.scale * 1.4426950408889634f;
   p.accumulate = d.accumulate;
   static DeviceOnce configured;
@@ -234,7 +234,7 @@ static int launch_attn(const AttnDesc& d, cudaStream_t stream) {
   return VC_OK;
 }
 
-int flash_attn_d64(const AttnDesc& d, cudaStream_t stream) {
+int flash_attn_d64(const vc_attn_desc& d, cudaStream_t stream) {
   VC_REQUIRE(d.q && d.k && d.v && d.out, "flash_attn: null pointer");
   VC_REQUIRE(d.Nq > 0 && d.Nk > 0 && d.B > 0 && d.heads > 0, "flash_attn: empty problem");
   VC_REQUIRE(d.ldq % 8 == 0 && d.ldk % 8 == 0 && d.ldv % 8 == 0 && d.ldo % 8 == 0, "flash_attn: pitches must be multiples of 8");

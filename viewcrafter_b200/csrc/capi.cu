@@ -24,29 +24,10 @@ const char* vc_last_error(void) { return vc::last_error(); }
 long long vc_launch_count(void) { return vc::g_launches.load(); }
 void vc_reset_launch_count(void) { vc::g_launches.store(0); }
 
-int vc_gemm_tap(const vc_gemm_desc* c, void* stream) {
-  if (!c) { set_error("vc_gemm_tap: null descriptor"); return VC_ERR_ARG; }
-  GemmDesc d;
-  d.a = H(c->a); d.lda = c->lda; d.a2 = H(c->a2); d.lda2 = c->lda2;
-  d.X = c->X; d.Y = c->Y; d.Z = c->Z; d.bx = c->bx; d.by = c->by;
-  d.K = c->K; d.K1 = c->K1; d.w = H(c->w); d.ldw = c->ldw; d.N = c->N; d.num_taps = c->num_taps;
-  for (int i = 0; i < 9; ++i) { d.tap_dx[i] = c->tap_dx[i]; d.tap_dy[i] = c->tap_dy[i]; }
-  d.out = HM(c->out); d.out_f32 = reinterpret_cast<float*>(c->out_f32); d.ldo = c->ldo;
-  d.bias = c->bias; d.bias_z_div = c->bias_z_div; d.res = H(c->res); d.ldr = c->ldr; d.geglu = c->geglu;
-  d.ln_stats = c->ln_stats; d.ln_colsum = c->ln_colsum; d.ln_part = c->ln_part; d.gn_part = c->gn_part; d.gn_sub = c->gn_sub;
-  d.ldo_y = c->ldo_y; d.ldo_z = c->ldo_z;
-  d.fp8 = c->fp8; d.w_scale = c->w_scale; d.a_amax = c->a_amax;
-  GemmPeerDesc pd;
-  if (c->peer && c->peer->mode) {
-    const vc_gemm_peer* q = c->peer;
-    pd.mode = q->mode; pd.world = q->world; pd.rank = q->rank; pd.B = q->B; pd.T = q->T; pd.HW = q->HW;
-    if (q->world < 1 || q->world > 8) { set_error("vc_gemm_tap: peer world %d out of range", q->world); return VC_ERR_ARG; }
-    for (int i = 0; i <= q->world; ++i) pd.f0[i] = q->f0[i];
-    for (int i = 0; i < q->world; ++i) pd.dst[i] = q->dst[i];
-    d.peer = &pd;
-  }
+int vc_gemm_tap(const vc_gemm_desc* d, void* stream) {
+  if (!d) { set_error("vc_gemm_tap: null descriptor"); return VC_ERR_ARG; }
   COUNT(1);
-  return gemm_tap(d, ST(stream));
+  return gemm_tap(*d, ST(stream));
 }
 int vc_gemm_tile_n(int32_t N, int32_t geglu) { return vc::pick_bn_public(N, geglu); }
 int vc_absmax_f16(const void* x1, int64_t rows, int32_t cols1, int32_t ld1, const void* x2, int32_t cols2, int32_t ld2, float* amax,
@@ -55,14 +36,10 @@ int vc_absmax_f16(const void* x1, int64_t rows, int32_t cols1, int32_t ld1, cons
   return absmax_f16(H(x1), rows, cols1, ld1, H(x2), cols2, ld2, amax, ST(stream));
 }
 
-int vc_flash_attn_d64(const vc_attn_desc* c, void* stream) {
-  if (!c) { set_error("vc_flash_attn_d64: null descriptor"); return VC_ERR_ARG; }
-  AttnDesc d;
-  d.q = H(c->q); d.ldq = c->ldq; d.k = H(c->k); d.ldk = c->ldk; d.v = H(c->v); d.ldv = c->ldv;
-  d.out = HM(c->out); d.ldo = c->ldo; d.B = c->B; d.heads = c->heads; d.Nq = c->Nq; d.Nk = c->Nk;
-  d.kv_batch_stride = c->kv_batch_stride; d.scale = c->scale; d.accumulate = c->accumulate;
+int vc_flash_attn_d64(const vc_attn_desc* d, void* stream) {
+  if (!d) { set_error("vc_flash_attn_d64: null descriptor"); return VC_ERR_ARG; }
   COUNT(1);
-  return flash_attn_d64(d, ST(stream));
+  return flash_attn_d64(*d, ST(stream));
 }
 
 int vc_temporal_attn(const void* q, const void* k, const void* v, int32_t ld, void* out, int32_t ldo, int32_t T, int64_t sites,
@@ -95,14 +72,9 @@ int vc_groupnorm_from_parts(const void* x1, int32_t C1, const vc_gn_part_geom* g
                             int32_t samples, int64_t rows_per_sample, const float* gamma, const float* beta, float eps, int32_t silu,
                             void* out, void* ws, size_t ws_bytes, void* stream) {
   if (!g1 || (x2 && !g2)) { set_error("vc_groupnorm_from_parts: null geometry"); return VC_ERR_ARG; }
-  auto conv = [](const vc_gn_part_geom* c) {
-    GnPartGeom g;
-    if (c) { g.part = c->part; g.n_chunks = c->n_chunks; g.sub = c->sub; g.rb_per_z = c->rb_per_z; g.samples_per_z = c->samples_per_z; g.rb_per_sample = c->rb_per_sample; }
-    return g;
-  };
   COUNT(x2 ? 3 : 2);
-  return groupnorm_from_parts(H(x1), C1, conv(g1), H(x2), C2, conv(g2), samples, rows_per_sample, gamma, beta, eps, silu, HM(out),
-                              reinterpret_cast<float*>(ws), ws_bytes, ST(stream));
+  return groupnorm_from_parts(H(x1), C1, *g1, H(x2), C2, x2 ? *g2 : *g1 /* not read without x2 */, samples, rows_per_sample, gamma, beta,
+                              eps, silu, HM(out), reinterpret_cast<float*>(ws), ws_bytes, ST(stream));
 }
 int vc_groupnorm_apply_parts(const void* x1, int32_t C1, int32_t samples, int64_t rows_per_sample, const float* parts, int32_t n_parts,
                              int64_t stat_rows, const float* gamma, const float* beta, float eps, int32_t silu, void* out, void* stream) {
@@ -188,23 +160,15 @@ int vc_small_linear_f32(const float* x, int32_t rows, int32_t K, const float* W,
 int vc_ddim_update(const float* x, const float* v_cond, const float* v_uncond, const float* noise, float* x_prev, float* pred_x0,
                    int64_t n, const vc_ddim_scalars* s, void* ws, void* stream) {
   if (!s) { set_error("vc_ddim_update: null scalars"); return VC_ERR_ARG; }
-  DdimStepScalars d;
-  d.cfg_scale = s->cfg_scale; d.guidance_rescale = s->guidance_rescale; d.sqrt_ac_t = s->sqrt_ac_t; d.sqrt_1mac_t = s->sqrt_1mac_t;
-  d.a_prev = s->a_prev; d.sigma_t = s->sigma_t; d.scale_t = s->scale_t; d.prev_scale_t = s->prev_scale_t; d.use_cfg = s->use_cfg;
-  d.reproducible = s->reproducible;
-  COUNT((d.use_cfg && d.guidance_rescale > 0.f) ? 2 : 1);
-  return ddim_update(x, v_cond, v_uncond, nullptr, 0.f, noise, x_prev, pred_x0, n, d, reinterpret_cast<double*>(ws), ST(stream));
+  COUNT((s->use_cfg && s->guidance_rescale > 0.f) ? 2 : 1);
+  return ddim_update(x, v_cond, v_uncond, nullptr, 0.f, noise, x_prev, pred_x0, n, *s, reinterpret_cast<double*>(ws), ST(stream));
 }
 int vc_ddim_update3(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img,
                     const float* noise, float* x_prev, float* pred_x0, int64_t n, const vc_ddim_scalars* s, void* ws, void* stream) {
   if (!s) { set_error("vc_ddim_update3: null scalars"); return VC_ERR_ARG; }
   if (!v_uncond_img) { set_error("vc_ddim_update3: null image-only branch"); return VC_ERR_ARG; }
-  DdimStepScalars d;
-  d.cfg_scale = s->cfg_scale; d.guidance_rescale = s->guidance_rescale; d.sqrt_ac_t = s->sqrt_ac_t; d.sqrt_1mac_t = s->sqrt_1mac_t;
-  d.a_prev = s->a_prev; d.sigma_t = s->sigma_t; d.scale_t = s->scale_t; d.prev_scale_t = s->prev_scale_t; d.use_cfg = s->use_cfg;
-  d.reproducible = s->reproducible;
-  COUNT((d.use_cfg && d.guidance_rescale > 0.f) ? 2 : 1);
-  return ddim_update(x, v_cond, v_uncond, v_uncond_img, cfg_img, noise, x_prev, pred_x0, n, d, reinterpret_cast<double*>(ws), ST(stream));
+  COUNT((s->use_cfg && s->guidance_rescale > 0.f) ? 2 : 1);
+  return ddim_update(x, v_cond, v_uncond, v_uncond_img, cfg_img, noise, x_prev, pred_x0, n, *s, reinterpret_cast<double*>(ws), ST(stream));
 }
 
 /* vc_enable_peer_access / vc_peer_exchange / vc_peer_groupnorm_stats: peer.cu */

@@ -188,8 +188,6 @@ __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
-// MUFU.EX2 + MUFU.RCP + 3 FP ops (an IEEE `x / y` costs ~10 more instructions per element and made GroupNorm+SiLU ALU-bound)
-__device__ __forceinline__ float silu_f(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
 // erf via Abramowitz-Stegun 7.1.26 (|abs err| < 1.5e-7, far below fp16 resolution): 1 MUFU.EX2 + 1 MUFU.RCP + 7 FMA
 __device__ __forceinline__ float erf_fast(float x) {
   const float ax = fabsf(x);

@@ -22,7 +22,7 @@
 //   tensor cores, this keeps every full-barrier wait within one phase of the barrier, which the parity waits require.
 // Tiles are ordered n-fastest so CTAs that run concurrently share A tiles in L2.
 //
-// FP8 variant (FP8 = true, GemmDesc::fp8): the weights are e4m3 (per-output-channel scales w_scale), a ring stage holds
+// FP8 variant (FP8 = true, vc_gemm_desc::fp8): the weights are e4m3 (per-output-channel scales w_scale), a ring stage holds
 // the fp16 A tile as before and the weight tile as 64-byte rows (64B swizzle).  The MMA warpgroup reads its A fragments from
 // the fp16 stage, scales them by 1 / s_a (s_a = a_amax / 448, one scale per GEMM call) and converts them to e4m3 in
 // registers (round to nearest, saturating), then issues wgmma m64nBNk32 e4m3 x e4m3 with A from registers.  A stays fp16 in
@@ -324,7 +324,7 @@ static int pick_bn(int N, int geglu, int fp8 = 0) {
 
 int pick_bn_public(int N, int geglu) { return pick_bn(N, geglu); }
 
-int gemm_tap(const GemmDesc& d, cudaStream_t stream) {
+int gemm_tap(const vc_gemm_desc& d, cudaStream_t stream) {
   VC_REQUIRE(d.a && d.w && (d.out || d.out_f32), "gemm_tap: null pointer");
   VC_REQUIRE(d.num_taps >= 1 && d.num_taps <= MAX_TAPS, "gemm_tap: num_taps=%d out of range", d.num_taps);
   VC_REQUIRE(d.bx * d.by == BM && d.bx >= 1, "gemm_tap: box %dx%d must cover 128 rows", d.bx, d.by);
@@ -393,9 +393,9 @@ int gemm_tap(const GemmDesc& d, cudaStream_t stream) {
   p.N = d.N; p.K = d.K; p.K1 = d.K1;
   p.num_taps = d.num_taps;
   for (int t = 0; t < d.num_taps; ++t) { p.tap_dx[t] = d.tap_dx[t]; p.tap_dy[t] = d.tap_dy[t]; }
-  p.out = d.out; p.out_f32 = d.out_f32; p.ldo = d.ldo;
+  p.out = static_cast<__half*>(d.out); p.out_f32 = static_cast<float*>(d.out_f32); p.ldo = d.ldo;
   p.bias = d.bias; p.bias_z_div = d.bias_z_div;
-  p.res = d.res; p.ldr = d.ldr;
+  p.res = static_cast<const __half*>(d.res); p.ldr = d.ldr;
   p.geglu = d.geglu;
   p.w_scale = d.w_scale; p.a_amax = d.a_amax;
   VC_REQUIRE((d.ln_stats == nullptr) == (d.ln_colsum == nullptr), "gemm_tap: ln_stats and ln_colsum go together");
@@ -436,8 +436,9 @@ int gemm_tap(const GemmDesc& d, cudaStream_t stream) {
   }
   if (d.peer && d.peer->mode) {
     // layout switch fused into the epilogue: per-rank destination maps (gemm_common.cuh: GemmPeer)
-    const GemmPeerDesc& q = *d.peer;
+    const vc_gemm_peer& q = *d.peer;
     VC_REQUIRE(q.mode == 1 || q.mode == 2, "gemm_tap: peer mode %d", q.mode);
+    // before anything indexes f0[world] / dst[rank]
     VC_REQUIRE(q.world >= 2 && q.world <= GEMM_PEER_MAX && q.rank >= 0 && q.rank < q.world, "gemm_tap: peer scatter supports 2..%d ranks", GEMM_PEER_MAX);
     VC_REQUIRE(p.out_tma && !d.geglu && !d.ln_part && d.ldo_y == 0 && d.ldo_z == 0, "gemm_tap: peer scatter needs the fp16 TMA-store epilogue");
     VC_REQUIRE(q.HW % q.world == 0 && q.f0[0] == 0 && q.f0[q.world] == q.T && q.B >= 1, "gemm_tap: peer scatter: bad frame / site split");

@@ -298,7 +298,7 @@ __global__ void __launch_bounds__(256) ddim_stats_kernel(const float* __restrict
 __global__ void ddim_apply_kernel(const float* __restrict__ x, const float* __restrict__ vc_, const float* __restrict__ vu,
                                   const float* __restrict__ vi, float cfg_img,
                                   const float* __restrict__ noise, float* __restrict__ x_prev, float* __restrict__ pred_x0,
-                                  long long n, DdimStepScalars s, const double* ws, int stat_blocks) {
+                                  long long n, vc_ddim_scalars s, const double* ws, int stat_blocks) {
   float factor = 1.f;
   if (s.use_cfg && s.guidance_rescale > 0.f) {
     __shared__ double tot[4];
@@ -333,7 +333,7 @@ __global__ void ddim_apply_kernel(const float* __restrict__ x, const float* __re
   }
 }
 int ddim_update(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img, const float* noise,
-                float* x_prev, float* pred_x0, long long n, const DdimStepScalars& s, double* ws, cudaStream_t stream) {
+                float* x_prev, float* pred_x0, long long n, const vc_ddim_scalars& s, double* ws, cudaStream_t stream) {
   VC_REQUIRE(x && v_cond && noise && x_prev && pred_x0 && ws && n > 1, "ddim_update: bad args");
   VC_REQUIRE(!s.use_cfg || v_uncond, "ddim_update: CFG needs the unconditional output");
   VC_REQUIRE(!v_uncond_img || s.use_cfg, "ddim_update: the image-only branch is only defined with CFG on");

@@ -5,17 +5,12 @@
 //   layernorm_rows : LayerNorm over the last dim, one warp per token row, values held in registers.
 // Reference semantics: lvdm/basics.py:76-87 (fp32 GroupNorm), attention.py:265,331 (eps 1e-6),
 // openaimodel3d.py:256-265 (5-D GroupNorm in TemporalConvBlock), torch.nn.LayerNorm (eps 1e-5).
-#include <cstdlib>
-
 #include "common.cuh"
 #include "kernels.h"
 
 namespace vc {
 
 static constexpr int GN_MAX_SPLITS = 512;
-#ifndef VC_GN_REVERSE
-#define VC_GN_REVERSE 1      // A/B switch: normalise pass walks its rows backwards (L2 reuse of the statistics pass)
-#endif
 
 size_t groupnorm_ws_bytes(int samples) { return (size_t)samples * GN_MAX_SPLITS * 64 * sizeof(float) + (size_t)samples * sizeof(unsigned int); }
 
@@ -100,21 +95,14 @@ __device__ __forceinline__ void gn_stats_dev(const __half* __restrict__ x1, cons
   __syncthreads();                                  // red[] may be rewritten by the caller's next use
 }
 
-#ifndef VC_SILU_TANH
-#define VC_SILU_TANH 1       // A/B switch: SiLU through ONE MUFU op (tanh.approx) instead of ex2 + rcp
-#endif
 // x * sigmoid(x) = h + h * tanh(h) with h = x / 2: one MUFU.TANH + 2 FP ops per element instead of MUFU.EX2 + MUFU.RCP + 3.  The
 // normalise pass issues 2 MUFU per element otherwise and is then bound by the 16-per-clock MUFU pipe rather than by HBM.  tanh.approx.f32 has a relative error of 2^-11 on tanh, i.e. an absolute error of
 // <= 2.4e-4 |x| on the result -- the size of the fp16 rounding the output gets anyway.
 __device__ __forceinline__ float gn_silu(float x) {
-#if VC_SILU_TANH
   const float h = 0.5f * x;
   float t;
   asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(h));
   return fmaf(h, t, h);
-#else
-  return silu_f(x);
-#endif
 }
 
 __device__ __forceinline__ uint4 gn_norm8(const uint4& u, const float (&sc)[8], const float (&sh)[8], int silu) {
@@ -169,15 +157,15 @@ __device__ __forceinline__ void gn_apply_dev(const __half* __restrict__ x1, cons
   }
   const GnThread t = gn_thread(x1, x2, g, split, sample, v, pl);
   const long long ostride = (long long)g.ppi * g.C;
-  // Walk the rows BACKWARDS (VC_GN_REVERSE): in the fused kernel the statistics pass streamed them forwards, so what the L2 still
+  // Walk the rows BACKWARDS: in the fused kernel the statistics pass streamed them forwards, so what the L2 still
   // holds is the tail of every CTA's slice; a second forward sweep is the worst case for an LRU-like cache, the reverse sweep meets
   // the resident lines first.
   // Software pipeline: the loads of the NEXT four rows are issued before the current four are normalised and stored, so up to eight
   // 16-byte loads per thread are in flight and the DRAM latency is covered when this pass is the only one (statistics from the
   // producing GEMM: no L2-resident tail to meet).
-  const long long ds = VC_GN_REVERSE ? -t.sstride : t.sstride, dd = VC_GN_REVERSE ? -ostride : ostride;
-  const __half* p = VC_GN_REVERSE ? t.src + (t.n - 1) * t.sstride : t.src;
-  __half* o = out + ((long long)sample * g.rows + t.orow0) * g.C + v * 8 + (VC_GN_REVERSE ? (t.n - 1) * ostride : 0);
+  const long long ds = -t.sstride, dd = -ostride;
+  const __half* p = t.src + (t.n - 1) * t.sstride;
+  __half* o = out + ((long long)sample * g.rows + t.orow0) * g.C + v * 8 + (t.n - 1) * ostride;
   long long left = t.n;
   uint4 cur[4], nxt[4];
   int ncur = left < 4 ? (int)left : 4;
@@ -403,7 +391,7 @@ int groupnorm_apply_leaves(const __half* x1, int C1, const __half* x2, int C2, i
 }
 
 // ------------------------------------------------------------------------------------------------
-// GroupNorm from the partial sums the producing GEMM left behind (GemmDesc::gn_part, gemm_common.cuh: gn_part_accumulate):
+// GroupNorm from the partial sums the producing GEMM left behind (vc_gemm_desc::gn_part, gemm_common.cuh: gn_part_accumulate):
 // the statistics pass over the activation disappears -- a small kernel folds the per-(32-row block, chunk, piece) records
 // (1.6 % of the activation's bytes) into per-(sample, split, group) sums in a fixed order, and gn_apply_kernel normalises in
 // one read + one write.  Reference semantics as above (basics.py:76-87, openaimodel3d.py:256-265).
@@ -467,7 +455,7 @@ __global__ void __launch_bounds__(1024) gn_part_finalize_kernel(GnFin f, float* 
 static constexpr int GN_PART_MAX_SPLITS = 64;          // per source
 size_t groupnorm_parts_ws_bytes(int samples) { return (size_t)samples * 2 * GN_PART_MAX_SPLITS * 64 * sizeof(float); }
 
-static int gn_part_plan(const GnPartGeom& g, int C_src, int samples, GnFin& f) {
+static int gn_part_plan(const vc_gn_part_geom& g, int C_src, int samples, GnFin& f) {
   VC_REQUIRE(g.part && g.n_chunks * 32 == C_src && (g.sub == 10 || g.sub == 8) && g.rb_per_sample >= 1 && g.samples_per_z >= 1 &&
              g.rb_per_z >= (long long)g.samples_per_z * g.rb_per_sample, "groupnorm_from_parts: bad partial-sum geometry");
   f.part = reinterpret_cast<const float2*>(g.part);
@@ -487,7 +475,7 @@ static int gn_part_plan(const GnPartGeom& g, int C_src, int samples, GnFin& f) {
 
 // The finalize step alone for ONE source: partial_ws[sample][split][64] = per-group (sum, sumsq) over the sample's rows ON THIS RANK,
 // from the producer's records -- the input of the cross-GPU statistics exchange (peer.cu: gn_peer_allreduce_kernel).
-int groupnorm_parts_to_partials(const GnPartGeom& g1, int C, int samples, float* partial_ws, size_t ws_bytes, int* splits_out,
+int groupnorm_parts_to_partials(const vc_gn_part_geom& g1, int C, int samples, float* partial_ws, size_t ws_bytes, int* splits_out,
                                 cudaStream_t stream) {
   VC_REQUIRE(partial_ws && splits_out && C % 32 == 0, "groupnorm_parts_to_partials: bad args");
   GnFin f;
@@ -502,7 +490,8 @@ int groupnorm_parts_to_partials(const GnPartGeom& g1, int C, int samples, float*
   return VC_OK;
 }
 
-int groupnorm_from_parts(const __half* x1, int C1, const GnPartGeom& g1, const __half* x2, int C2, const GnPartGeom& g2, int samples,
+int groupnorm_from_parts(const __half* x1, int C1, const vc_gn_part_geom& g1, const __half* x2, int C2, const vc_gn_part_geom& g2,
+                         int samples,
                          long long rows_per_sample, const float* gamma, const float* beta, float eps, int silu, __half* out, float* ws,
                          size_t ws_bytes, cudaStream_t stream) {
   VC_REQUIRE(out && gamma && beta && ws, "groupnorm_from_parts: null pointer");
@@ -637,7 +626,7 @@ int layernorm_rows(const __half* x, long long rows, int C, const float* gamma, c
 }
 
 // Statistics half of LayerNorm: stats[row] = (mean, rstd).  The normalisation itself is folded into the consuming GEMM's
-// epilogue (GemmDesc::ln_stats), which turns LayerNorm from a read + write pass into this read-only pass.
+// epilogue (vc_gemm_desc::ln_stats), which turns LayerNorm from a read + write pass into this read-only pass.
 // One warp per group of 4 rows, every lane keeps 4 independent 16-byte loads in flight; sums are taken about a per-row
 // pivot (the row's first element) so the one-pass variance does not cancel when |mean| >> std.  ~40 registers: 48+ warps
 // per SM (the register-resident two-pass kernel above runs at 16 warps per SM).
@@ -761,7 +750,7 @@ __global__ void __launch_bounds__(256) ln_stats_unrolled_kernel(const __half* __
   }
 }
 
-// (mean, rstd) per row from the per-32-column partial sums a producing GEMM left in parts[C/32][rows] (GemmDesc::ln_part):
+// (mean, rstd) per row from the per-32-column partial sums a producing GEMM left in parts[C/32][rows] (vc_gemm_desc::ln_part):
 // reads C/32 * 8 bytes per row instead of 2 C bytes -- the LayerNorm statistics pass without re-reading the activation.
 __global__ void __launch_bounds__(256) ln_finalize_kernel(const float2* __restrict__ parts, long long rows, int nchunks, float invC, float eps,
                                                           float2* __restrict__ stats) {
@@ -794,12 +783,10 @@ int layernorm_stats(const __half* x, long long rows, int C, float eps, float* st
   long long blocks = (rows + 4 * wpb - 1) / (4 * wpb);
   const long long cap = (long long)sm_count() * 8;              // 8 x 256 threads = 64 warps per SM
   if (blocks > cap) blocks = cap;
-  static int unroll = -1;                       // VC_LN_STATS_UNROLL=0: the rolled loop
-  if (unroll < 0) { const char* e = getenv("VC_LN_STATS_UNROLL"); unroll = (e && e[0] == '0') ? 0 : 1; }
   const int iters = (C / 8 + 31) / 32;
-  if (unroll && iters <= 2)
+  if (iters <= 2)
     ln_stats_unrolled_kernel<2><<<(unsigned)blocks, wpb * 32, 0, stream>>>(x, rows, C, eps, reinterpret_cast<float2*>(stats));
-  else if (unroll && iters <= 4)
+  else if (iters <= 4)
     ln_stats_unrolled_kernel<4><<<(unsigned)blocks, wpb * 32, 0, stream>>>(x, rows, C, eps, reinterpret_cast<float2*>(stats));
   else
     ln_stats_kernel<<<(unsigned)blocks, wpb * 32, 0, stream>>>(x, rows, C, eps, reinterpret_cast<float2*>(stats));

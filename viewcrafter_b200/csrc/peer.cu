@@ -236,8 +236,6 @@ __global__ void __launch_bounds__(512) peer_leaves_kernel(const float* __restric
 }  // namespace vc
 
 // ------------------------------------------------------------------------------------------------------------------
-#include "../../include/vc_b200.h"
-
 namespace vc {
 int groupnorm_stats_partials(const __half* x1, int C1, int samples, long long rows_per_sample, float* partial_ws, size_t ws_bytes,
                              int* splits_out, cudaStream_t stream);
@@ -376,10 +374,7 @@ int vc_peer_finish_scatter(const vc_peer_comm* c, const vc_gn_part_geom* geom, i
   int splits = 0, B = 0;
   if (geom) {
     VC_REQUIRE(samples >= 1 && samples <= c->Bmax, "peer_finish_scatter: samples %d exceed Bmax %d", samples, c->Bmax);
-    GnPartGeom g;
-    g.part = geom->part; g.n_chunks = geom->n_chunks; g.sub = geom->sub; g.rb_per_z = geom->rb_per_z; g.samples_per_z = geom->samples_per_z;
-    g.rb_per_sample = geom->rb_per_sample;
-    rc = groupnorm_parts_to_partials(g, C, samples, reinterpret_cast<float*>(ws), ws_bytes, &splits, reinterpret_cast<cudaStream_t>(stream));
+    rc = groupnorm_parts_to_partials(*geom, C, samples, reinterpret_cast<float*>(ws), ws_bytes, &splits, reinterpret_cast<cudaStream_t>(stream));
     if (rc) return rc;
     B = samples;
   }

@@ -189,17 +189,6 @@ def absmax(x: torch.Tensor, x2: Optional[torch.Tensor] = None, out: Optional[tor
     return out
 
 
-def _set_w(d: GemmDesc, w, amax: Optional[torch.Tensor]):
-    """Point the descriptor at the weight: fp16 [rows, K], or an Fp8Weight with the activation's absmax scalar."""
-    if isinstance(w, Fp8Weight):
-        assert amax is not None and w.q.is_cuda and w.q.dtype == torch.float8_e4m3fn
-        d.w, d.ldw = w.q.data_ptr(), w.q.stride(0)
-        d.fp8, d.w_scale, d.a_amax = 1, w.scale.data_ptr(), amax.data_ptr()
-    else:
-        _chk16(w, "gemm.w")
-        d.w, d.ldw = w.data_ptr(), w.stride(0)
-
-
 # ----------------------------------------------------------------------------------------------------
 # tensor-core ops
 # ----------------------------------------------------------------------------------------------------
@@ -207,7 +196,6 @@ def _gemm(desc: GemmDesc):
     check(_lib.load().vc_gemm_tap(C.byref(desc), _stream()), "vc_gemm_tap")
 
 
-LN_FROM_PRODUCER = os.environ.get("VC_LN_FROM_PRODUCER", "1") != "0"   # A/B switch: LayerNorm statistics from the producing GEMM's epilogue
 # GroupNorm statistics from the producing GEMM's epilogue (GemmDesc.gn_part): 0 = off (statistics pass inside the GroupNorm kernel),
 # 1 = producers with a long reduction only (3x3 / temporal / stride-2 convs: the extra epilogue work hides under the MMAs), 2 = every producer
 GN_FROM_PRODUCER = int(os.environ.get("VC_GN_FROM_PRODUCER", "1"))
@@ -277,19 +265,6 @@ class GnPart:
         return None
 
 
-def _gn_part_alloc(d: GemmDesc, device):
-    """Allocate the record buffer for the GEMM described by d and hook it up; returns the GnPart (or None if N does not qualify)."""
-    N = d.N
-    if N % 32 != 0 or N % GN_SUB != 0 or d.geglu or not d.out:
-        return None
-    tx, ty = -(-d.X // d.bx), -(-d.Y // d.by)
-    m_tiles = tx * ty * d.Z
-    n_rb = m_tiles * 4                                          # one record row per 32-row block
-    part = torch.empty((n_rb, N // 32, 4, 2), device=device, dtype=torch.float32)
-    d.gn_part, d.gn_sub = part.data_ptr(), GN_SUB
-    return GnPart(part, N // 32, GN_SUB, tx * ty * 4, d.X * d.Y, d.Z, linear=(d.by == 1 and d.bx == 128 and (d.Y == 1 or d.X % 128 == 0)))
-
-
 def _want_gn(gn_out: bool, k_iters: int) -> bool:
     # reproducible mode never reads the producer's sums (their order follows the GEMM's tiling of the whole batch)
     return bool(gn_out) and not REPRODUCIBLE and (GN_FROM_PRODUCER >= 2 or (GN_FROM_PRODUCER == 1 and k_iters >= 12))
@@ -300,6 +275,92 @@ def gn_part_of(t):
 
 
 gn_from_parts_calls = 0      # GroupNorms that took their statistics from a producer's partial sums (introspection / tests)
+
+
+def _tap_gemm(who: str, x: torch.Tensor, w, X: int, Y: int, Z: int, bx: int, by: int, taps, x2: Optional[torch.Tensor] = None,
+              amax: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None, out_f32: bool = False, ldo: Optional[int] = None,
+              ldo_y: int = 0, ldo_z: int = 0, bias: Optional[torch.Tensor] = None, bias_z_div: int = 0, res: Optional[torch.Tensor] = None,
+              geglu: bool = False, ln=None, ln_out: bool = False, gn_out: bool = False, peer=None):
+    """Launch one tap-GEMM: out[row] = sum over taps (dx, dy) of [x|x2][row shifted by (dx, dy) in the (X, Y, Z) grid] @ w_tap.T, then
+    the epilogue options of linear().  w: fp16 [len(taps) * N, K] or an Fp8Weight (amax: the absmax of [x|x2], computed here if None).
+    out: written with row pitch ldo (default out.stride(0)) and optional Y / Z pitches; allocated [M, N] if None.  Returns what linear()
+    returns."""
+    _chk16(x, f"{who}.x")
+    fp8 = isinstance(w, Fp8Weight)
+    if fp8 and peer is not None:
+        raise VcError(f"{who}: FP8 weights do not support the multi-GPU peer-scatter epilogue")
+    M, K1 = x.shape
+    K = w.shape[1]
+    N = w.shape[0] // len(taps)
+    n_out = N // 2 if geglu else N
+    d = GemmDesc()
+    d.a, d.lda = x.data_ptr(), x.stride(0)
+    if x2 is not None:
+        d.a2, d.lda2 = x2.data_ptr(), x2.stride(0)
+        assert K1 + x2.shape[1] == K
+    else:
+        assert K1 == K, (K1, K)
+    d.X, d.Y, d.Z, d.bx, d.by = X, Y, Z, bx, by
+    d.K, d.K1, d.N, d.num_taps = K, K1, N, len(taps)
+    for t, (dx, dy) in enumerate(taps):
+        d.tap_dx[t], d.tap_dy[t] = dx, dy
+    if fp8:
+        if amax is None:
+            amax = absmax(x, x2)
+        assert w.q.is_cuda and w.q.dtype == torch.float8_e4m3fn
+        d.w, d.ldw = w.q.data_ptr(), w.q.stride(0)
+        d.fp8, d.w_scale, d.a_amax = 1, w.scale.data_ptr(), amax.data_ptr()
+    else:
+        _chk16(w, "gemm.w")
+        d.w, d.ldw = w.data_ptr(), w.stride(0)      # w may be a column slice of a wider matrix (e.g. K of a fused QK)
+    if peer is not None:
+        assert out is None and not geglu and not out_f32 and not ln_out and M == peer.rows_in and N == peer.C
+        peer.attach(d)                              # the output goes to the peers' receive buffers
+    else:
+        if out is None:
+            out = torch.empty((M, n_out), device=x.device, dtype=torch.float32 if out_f32 else torch.float16)
+        if out_f32:
+            d.out_f32 = out.data_ptr()
+        else:
+            d.out = out.data_ptr()
+        d.ldo = out.stride(0) if ldo is None else ldo
+        d.ldo_y, d.ldo_z = ldo_y, ldo_z
+    d.bias, d.bias_z_div = _ptr(bias), bias_z_div
+    if res is not None:
+        d.res, d.ldr = res.data_ptr(), res.stride(0)
+    d.geglu = int(geglu)
+    if ln is not None:
+        stats, colsum = ln
+        assert stats.shape == (M, 2) and stats.dtype == torch.float32 and stats.is_contiguous()
+        assert colsum.shape == (N,) and colsum.dtype == torch.float32 and colsum.is_contiguous()
+        d.ln_stats, d.ln_colsum = stats.data_ptr(), colsum.data_ptr()
+    # GroupNorm records: a frames -> sites switch always leaves them (the cross-rank GroupNorm sums come from them); a local output
+    # when its GroupNorm reads them (gn_out) and the reduction is long enough for the extra epilogue work to hide under the MMAs
+    if peer is not None:
+        want_gn = peer.to_sites and not REPRODUCIBLE
+    else:
+        want_gn = _want_gn(gn_out, len(taps) * -(-K // 64)) and not out_f32 and out.is_contiguous()
+    part = None
+    if want_gn and N % 32 == 0 and N % GN_SUB == 0 and not geglu:
+        tx, ty = -(-X // bx), -(-Y // by)
+        buf = torch.empty((tx * ty * Z * 4, N // 32, 4, 2), device=x.device, dtype=torch.float32)     # one record row per 32-row block
+        d.gn_part, d.gn_sub = buf.data_ptr(), GN_SUB
+        part = GnPart(buf, N // 32, GN_SUB, tx * ty * 4, X * Y, Z, linear=(by == 1 and bx == 128 and (Y == 1 or X % 128 == 0)))
+    ln_parts = None
+    if ln_out and n_out % 32 == 0 and not geglu and not out_f32 and out.is_contiguous():
+        ln_parts = torch.empty((n_out // 32, M, 2), device=x.device, dtype=torch.float32)
+        d.ln_part = ln_parts.data_ptr()
+    _gemm(d)
+    if peer is not None:
+        return peer.finish(part)
+    out._vc_gn = part
+    if not ln_out:
+        return out
+    if ln_parts is None:                            # an output the epilogue cannot gather LayerNorm sums for: a statistics pass
+        return out, layernorm_stats(out)
+    st = torch.empty((M, 2), device=x.device, dtype=torch.float32)
+    check(_lib.load().vc_layernorm_stats_from_parts(ln_parts.data_ptr(), M, n_out, 1e-5, st.data_ptr(), _stream()), "vc_layernorm_stats_from_parts")
+    return out, st
 
 
 def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, res: Optional[torch.Tensor] = None,
@@ -313,65 +374,8 @@ def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None
     peer: a parallel.PeerFrameComm.scatter_plan(): the epilogue stores y into the other ranks' receive buffers (multi-GPU layout switch
     fused into the GEMM); returns the switched tensor.
     w may be an Fp8Weight (FP8 mode): the absmax of [x|x2] is computed first and the GEMM runs e4m3 x e4m3."""
-    _chk16(x, "linear.x")
-    fp8 = isinstance(w, Fp8Weight)
-    if fp8 and peer is not None:
-        raise VcError("linear: FP8 weights do not support the multi-GPU peer-scatter epilogue")
-    M, K1 = x.shape
-    N, K = w.shape
-    n_out = N // 2 if geglu else N
-    if peer is not None:
-        assert out is None and not geglu and not out_f32 and not ln_out and M == peer.rows_in and N == peer.C
-        out = x.new_empty((0, N))                      # placeholder: the descriptor's output is set by the plan
-    if out is None:
-        out = torch.empty((M, n_out), device=x.device, dtype=torch.float32 if out_f32 else torch.float16)
-    d = GemmDesc()
-    d.a, d.lda = x.data_ptr(), x.stride(0)
-    if x2 is not None:
-        d.a2, d.lda2 = x2.data_ptr(), x2.stride(0)
-        assert K1 + x2.shape[1] == K
-    else:
-        assert K1 == K, (K1, K)
-    d.X, d.Y, d.Z, d.bx, d.by = M, 1, 1, 128, 1
-    d.K, d.K1, d.N, d.num_taps = K, K1, N, 1
-    _set_w(d, w, absmax(x, x2) if fp8 else None)         # w may be a column slice of a wider matrix (e.g. K of a fused QK)
-    if out_f32:
-        d.out_f32 = out.data_ptr()
-    else:
-        d.out = out.data_ptr()
-    d.ldo = out.stride(0)
-    d.bias = _ptr(bias)
-    if res is not None:
-        d.res, d.ldr = res.data_ptr(), res.stride(0)
-    d.geglu = int(geglu)
-    if ln is not None:
-        stats, colsum = ln
-        assert stats.shape == (M, 2) and stats.dtype == torch.float32 and stats.is_contiguous()
-        assert colsum.shape == (N,) and colsum.dtype == torch.float32 and colsum.is_contiguous()
-        d.ln_stats, d.ln_colsum = stats.data_ptr(), colsum.data_ptr()
-    if peer is not None:
-        return _peer_gemm(d, peer, x.device)
-    out._vc_gn = _gn_part_alloc(d, x.device) if (_want_gn(gn_out, -(-K // 64)) and not out_f32 and not geglu and out.is_contiguous()) else None
-    if not ln_out:
-        _gemm(d)
-        return out
-    if not (LN_FROM_PRODUCER and n_out % 32 == 0 and not geglu and not out_f32 and out.is_contiguous()):
-        _gemm(d)
-        return out, layernorm_stats(out)
-    parts = torch.empty((n_out // 32, M, 2), device=x.device, dtype=torch.float32)
-    d.ln_part = parts.data_ptr()
-    _gemm(d)
-    st = torch.empty((M, 2), device=x.device, dtype=torch.float32)
-    check(_lib.load().vc_layernorm_stats_from_parts(parts.data_ptr(), M, n_out, 1e-5, st.data_ptr(), _stream()), "vc_layernorm_stats_from_parts")
-    return out, st
-
-
-def _peer_gemm(d: GemmDesc, peer, device):
-    """Launch a GEMM whose epilogue performs a multi-GPU layout switch (parallel._ScatterPlan) and complete the switch."""
-    peer.attach(d)
-    part = _gn_part_alloc(d, device) if (peer.to_sites and not REPRODUCIBLE) else None      # frames -> sites: the cross-rank GroupNorm sums come from these records
-    _gemm(d)
-    return peer.finish(part)
+    return _tap_gemm("linear", x, w, x.shape[0], 1, 1, 128, 1, ((0, 0),), x2=x2, out=out, out_f32=out_f32, bias=bias, res=res,
+                     geglu=geglu, ln=ln, ln_out=ln_out, gn_out=gn_out, peer=peer)
 
 
 def _conv_box(H: int, W: int):
@@ -383,53 +387,16 @@ def _conv_box(H: int, W: int):
     return W, 128 // W
 
 
+_TAPS_3X3 = tuple((t % 3 - 1, t // 3 - 1) for t in range(9))     # tap = ky * 3 + kx (pack_conv3x3)
+
+
 def conv3x3(x: torch.Tensor, frames: int, H: int, W: int, w9: torch.Tensor, bias: Optional[torch.Tensor] = None,
             res: Optional[torch.Tensor] = None, x2: Optional[torch.Tensor] = None, bias_z_div: int = 0,
             out_f32: bool = False, out: Optional[torch.Tensor] = None, gn_out: bool = False, peer=None) -> torch.Tensor:
     """3x3 / stride 1 / pad 1 convolution on [frames*H*W, Cin] rows; w9 = pack_conv3x3(weight).  gn_out / peer: see linear()."""
-    _chk16(x, "conv3x3.x")
-    fp8 = isinstance(w9, Fp8Weight)
-    if fp8 and peer is not None:
-        raise VcError("conv3x3: FP8 weights do not support the multi-GPU peer-scatter epilogue")
-    M, K1 = x.shape
-    assert M == frames * H * W, (M, frames, H, W)
-    K = w9.shape[1]
-    N = w9.shape[0] // 9
-    if peer is not None:
-        assert out is None and not out_f32 and M == peer.rows_in and N == peer.C
-        out = x.new_empty((0, N))
-    if out is None:
-        out = torch.empty((M, N), device=x.device, dtype=torch.float32 if out_f32 else torch.float16)
-    d = GemmDesc()
-    d.a, d.lda = x.data_ptr(), x.stride(0)
-    if x2 is not None:
-        d.a2, d.lda2 = x2.data_ptr(), x2.stride(0)
-        assert K1 + x2.shape[1] == K
-    else:
-        assert K1 == K, (K1, K)
-    d.X, d.Y, d.Z = W, H, frames
-    d.bx, d.by = _conv_box(H, W)
-    d.K, d.K1, d.N, d.num_taps = K, K1, N, 9
-    _set_w(d, w9, absmax(x, x2) if fp8 else None)
-    for t in range(9):
-        d.tap_dx[t] = t % 3 - 1
-        d.tap_dy[t] = t // 3 - 1
-    if out_f32:
-        d.out_f32 = out.data_ptr()
-    else:
-        d.out = out.data_ptr()
-    d.ldo = out.stride(0)
-    d.bias, d.bias_z_div = _ptr(bias), bias_z_div
-    if res is not None:
-        d.res, d.ldr = res.data_ptr(), res.stride(0)
-    if peer is not None:
-        return _peer_gemm(d, peer, x.device)
-    out._vc_gn = _gn_part_alloc(d, x.device) if (_want_gn(gn_out, 9 * -(-K // 64)) and not out_f32 and out.is_contiguous()) else None
-    _gemm(d)
-    return out
-
-
-UPCONV_FUSED = os.environ.get("VC_UPCONV_FUSED", "1") != "0"     # A/B switch: 0 = materialise the upsampled tensor, then a 9-tap conv
+    assert x.shape[0] == frames * H * W, (x.shape[0], frames, H, W)
+    return _tap_gemm("conv3x3", x, w9, W, H, frames, *_conv_box(H, W), _TAPS_3X3, x2=x2, out=out, out_f32=out_f32, bias=bias,
+                     bias_z_div=bias_z_div, res=res, gn_out=gn_out, peer=peer)
 
 
 def pack_upconv3x3(w: torch.Tensor):
@@ -438,8 +405,6 @@ def pack_upconv3x3(w: torch.Tensor):
     with the 3x3 taps that land on the same source pixel pre-summed (in fp32, then rounded to fp16): rows a=0: {W[0]}, {W[1]+W[2]};
     a=1: {W[0]+W[1]}, {W[2]}; columns alike.  4/9 of the FLOPs, and the 4x larger upsampled tensor is never materialised.
     Returns 4 packed tensors [(4*Cout), Cin] (tap = r*2 + c) for parities (0,0), (0,1), (1,0), (1,1)."""
-    if not UPCONV_FUSED:
-        return pack_conv3x3(w.detach())
     w32 = w.detach().float()
     co, ci = w32.shape[0], w32.shape[1]
     rows = {0: [w32[:, :, 0], w32[:, :, 1] + w32[:, :, 2]], 1: [w32[:, :, 0] + w32[:, :, 1], w32[:, :, 2]]}     # [co, ci, kx] each
@@ -457,64 +422,26 @@ def pack_upconv3x3(w: torch.Tensor):
 
 def upconv3x3(x: torch.Tensor, frames: int, H: int, W: int, packs, bias: Optional[torch.Tensor] = None) -> torch.Tensor:
     """conv3x3(upsample2x(x)) on [frames*H*W, Cin] rows -> [frames*2H*2W, Cout]; packs = pack_upconv3x3(weight)."""
-    _chk16(x, "upconv3x3.x")
-    if isinstance(packs, torch.Tensor):            # VC_UPCONV_FUSED=0: plain 9-tap weights
-        return conv3x3(upsample2x(x, frames, H, W), frames, 2 * H, 2 * W, packs, bias=bias)
-    M, K = x.shape
-    assert M == frames * H * W
+    assert x.shape[0] == frames * H * W
     N = packs[0].shape[0] // 4
     assert N % 32 == 0, "upconv3x3 writes through the TMA-store epilogue: Cout must be a multiple of 32"
     out = torch.empty((frames * 4 * H * W, N), device=x.device, dtype=torch.float16)
     amax = absmax(x) if isinstance(packs[0], Fp8Weight) else None      # FP8: one activation scale for the four parities
     for a in (0, 1):
         for b in (0, 1):
-            w4 = packs[a * 2 + b]
-            d = GemmDesc()
-            d.a, d.lda = x.data_ptr(), x.stride(0)
-            d.X, d.Y, d.Z = W, H, frames
-            d.bx, d.by = _conv_box(H, W)
-            d.K, d.K1, d.N, d.num_taps = K, K, N, 4
-            _set_w(d, w4, amax)
-            for t in range(4):
-                d.tap_dx[t] = (t % 2) + b - 1
-                d.tap_dy[t] = (t // 2) + a - 1
-            d.out = out.data_ptr() + ((a * 2 * W + b) * N) * 2          # pixel (a, b) of the large image
-            d.ldo, d.ldo_y, d.ldo_z = 2 * N, 4 * W * N, 4 * W * H * N   # every second pixel along x and y
-            d.bias = _ptr(bias)
-            _gemm(d)
+            taps = tuple((t % 2 + b - 1, t // 2 + a - 1) for t in range(4))
+            # rows from pixel (a, b) of the large image on, every second pixel along x and y
+            _tap_gemm("upconv3x3", x, packs[a * 2 + b], W, H, frames, *_conv_box(H, W), taps, amax=amax, out=out[a * 2 * W + b:],
+                      ldo=2 * N, ldo_y=4 * W * N, ldo_z=4 * W * H * N, bias=bias)
     return out
 
 
 def conv_temporal(x: torch.Tensor, B: int, T: int, HW: int, w3: torch.Tensor, bias: Optional[torch.Tensor] = None,
                   res: Optional[torch.Tensor] = None, gn_out: bool = False, peer=None) -> torch.Tensor:
     """Conv3d (3,1,1) pad (1,0,0) on [(B T) HW, C] rows: three row-shifted GEMM taps; batches never mix (Z = B).  gn_out: see linear()."""
-    _chk16(x, "conv_temporal.x")
-    fp8 = isinstance(w3, Fp8Weight)
-    if fp8 and peer is not None:
-        raise VcError("conv_temporal: FP8 weights do not support the multi-GPU peer-scatter epilogue")
-    M, K = x.shape
-    assert M == B * T * HW
-    N = w3.shape[0] // 3
-    if peer is not None:
-        assert M == peer.rows_in and N == peer.C
-    out = torch.empty((0 if peer is not None else M, N), device=x.device, dtype=torch.float16)
-    d = GemmDesc()
-    d.a, d.lda = x.data_ptr(), x.stride(0)
-    d.X, d.Y, d.Z, d.bx, d.by = T * HW, 1, B, 128, 1
-    d.K, d.K1, d.N, d.num_taps = K, K, N, 3
-    _set_w(d, w3, absmax(x) if fp8 else None)
-    for t in range(3):
-        d.tap_dx[t] = (t - 1) * HW
-        d.tap_dy[t] = 0
-    d.out, d.ldo = out.data_ptr(), out.stride(0)
-    d.bias = _ptr(bias)
-    if res is not None:
-        d.res, d.ldr = res.data_ptr(), res.stride(0)
-    if peer is not None:
-        return _peer_gemm(d, peer, x.device)
-    out._vc_gn = _gn_part_alloc(d, x.device) if _want_gn(gn_out, 3 * -(-K // 64)) else None
-    _gemm(d)
-    return out
+    assert x.shape[0] == B * T * HW
+    return _tap_gemm("conv_temporal", x, w3, T * HW, 1, B, 128, 1, tuple(((t - 1) * HW, 0) for t in range(3)), bias=bias, res=res,
+                     gn_out=gn_out, peer=peer)
 
 
 def flash_attn(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, B: int, Nq: int, Nk: int, heads: int,

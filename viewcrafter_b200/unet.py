@@ -30,15 +30,16 @@ def _zero(m: nn.Module) -> nn.Module:
     return m
 
 
-_LN_FOLD = os.environ.get("VC_LN_FOLD", "1") != "0"   # fold norm1/2/3 into their consumer GEMMs (A/B switch, read at import)
+def _ln_linear(Q: dict, x: torch.Tensor, st: torch.Tensor, name: str, **kw) -> torch.Tensor:
+    """LayerNorm -> Linear of a transformer block, the LayerNorm folded into the GEMM (ops.fold_layernorm).  `st`: the (mean, rstd) of x
+    that the GEMM producing x gathered (ops.linear(..., ln_out=True))."""
+    return ops.linear(x, Q[name], bias=Q[name + "_b"], ln=(st, Q[name + "_cs"]), **kw)
 
 
-def _ln_linear(Q: dict, x: torch.Tensor, name: str, ln: str, st=None, **kw) -> torch.Tensor:
-    """LayerNorm -> Linear of a transformer block: folded (row statistics + GEMM epilogue) or as two passes.  `st`: the (mean, rstd)
-    of x if the GEMM that produced x already gathered them (ops.linear(..., ln_out=True)); otherwise a statistics pass reads x."""
-    if Q[name + "_cs"] is not None:
-        return ops.linear(x, Q[name], bias=Q[name + "_b"], ln=(st if st is not None else ops.layernorm_stats(x), Q[name + "_cs"]), **kw)
-    return ops.linear(ops.layernorm(x, *Q[ln]), Q[name], bias=Q[name + "_b"], **kw)
+def _ff(Q: dict, x: torch.Tensor, st: torch.Tensor, last: bool):
+    """norm3 -> GEGLU -> FF2 (+ residual) of a transformer block: (y, LayerNorm statistics of y), or (y, None) after the last block."""
+    y = ops.linear(_ln_linear(Q, x, st, "ff1", geglu=True), Q["ff2_w"], bias=Q["ff2_b"], res=x, ln_out=not last)
+    return (y, None) if last else y
 
 
 def _fp8(w, taps: int = 1) -> "ops.Fp8Weight":
@@ -77,7 +78,7 @@ def _fp8_module(P: dict) -> dict:
     elif k == "D":
         Q8["w"] = _fp8(P["w"])
     elif k == "U":
-        Q8["w"] = [_fp8(w, 4) for w in P["w"]] if isinstance(P["w"], list) else _fp8(P["w"], 9)
+        Q8["w"] = [_fp8(w, 4) for w in P["w"]]
     return Q8                                               # "C": the first conv stays fp16
 
 
@@ -375,15 +376,10 @@ class UNetModel(nn.Module):
             Q = {}
             # norm1/2/3 feed exactly one linear each (attention.py:283-292): fold them into it -- the GEMM reads the raw
             # residual stream and its epilogue applies (mean, rstd); LayerNorm shrinks to a read-only statistics pass.
-            # VC_LN_FOLD=0 keeps the separate LayerNorm pass (A/B switch).
             n1, n2, n3 = ((ln.weight.detach(), ln.bias.detach()) for ln in (b.norm1, b.norm2, b.norm3))
             a1, a2 = b.attn1, b.attn2
             cat = lambda *ws: torch.cat(ws, 0).detach()
-            if _LN_FOLD:
-                fold = ops.fold_layernorm
-            else:
-                fold = lambda w, g, bta: (ops.pack_linear(w), None, None)
-                Q["ln1"], Q["ln2"], Q["ln3"] = ((f(g), f(bta)) for g, bta in (n1, n2, n3))
+            fold = ops.fold_layernorm
             Q["qkv1"], Q["qkv1_cs"], Q["qkv1_b"] = fold(cat(a1.to_q.weight, a1.to_k.weight, a1.to_v.weight), *n1)
             Q["o1_w"], Q["o1_b"] = ops.pack_linear(a1.to_out[0].weight.detach()), f(a1.to_out[0].bias)
             if m.kind == "T":
@@ -394,11 +390,7 @@ class UNetModel(nn.Module):
                 if hasattr(a2, "to_k_ip"):
                     Q["kv_img"] = torch.cat([a2.to_k_ip.weight, a2.to_v_ip.weight], 0).detach().to(torch.float16).contiguous()
             Q["o2_w"], Q["o2_b"] = ops.pack_linear(a2.to_out[0].weight.detach()), f(a2.to_out[0].bias)
-            if _LN_FOLD:
-                Q["ff1"], Q["ff1_b"], Q["ff1_cs"] = ops.pack_geglu_ln(b.ff.net[0].proj.weight.detach(), b.ff.net[0].proj.bias.detach(), *n3)
-            else:
-                Q["ff1"], Q["ff1_b"] = ops.pack_geglu(b.ff.net[0].proj.weight.detach(), b.ff.net[0].proj.bias.detach())
-                Q["ff1_cs"] = None
+            Q["ff1"], Q["ff1_b"], Q["ff1_cs"] = ops.pack_geglu_ln(b.ff.net[0].proj.weight.detach(), b.ff.net[0].proj.bias.detach(), *n3)
             Q["ff2_w"], Q["ff2_b"] = ops.pack_linear(b.ff.net[2].weight.detach()), f(b.ff.net[2].bias)
             blocks.append(Q)
         P["blocks"] = blocks
@@ -489,19 +481,15 @@ class UNetModel(nn.Module):
         Bc = 1 if expand else B
         BT, HW, heads = Bc * T, H * W, P["heads"]
         C = heads * 64
-        fold = _LN_FOLD
-        x = ops.linear(ops.groupnorm(h, BT, *P["gn"], 1e-6, False), P["in_w"], bias=P["in_b"], ln_out=fold)
-        x, st = x if fold else (x, None)
+        x, st = ops.linear(ops.groupnorm(h, BT, *P["gn"], 1e-6, False), P["in_w"], bias=P["in_b"], ln_out=True)
         for Q in P["blocks"]:
-            qkv = _ln_linear(Q, x, "qkv1", "ln1", st)
+            qkv = _ln_linear(Q, x, st, "qkv1")
             a = ops.flash_attn(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], BT, HW, HW, heads)
-            x = ops.linear(a, Q["o1_w"], bias=Q["o1_b"], res=x, ln_out=fold)
-            x, st = x if fold else (x, None)
+            x, st = ops.linear(a, Q["o1_w"], bias=Q["o1_b"], res=x, ln_out=True)
             if expand:
-                x, h = torch.cat([x] * B, 0), torch.cat([h] * B, 0)
-                st = torch.cat([st] * B, 0) if st is not None else None
+                x, h, st = torch.cat([x] * B, 0), torch.cat([h] * B, 0), torch.cat([st] * B, 0)
                 expand, Bc, BT = False, B, B * T
-            q = _ln_linear(Q, x, "q2", "ln2", st)
+            q = _ln_linear(Q, x, st, "q2")
             a = torch.empty_like(q)
             for b in range(Bc):
                 rows = slice(b * T * HW, (b + 1) * T * HW)
@@ -513,12 +501,8 @@ class UNetModel(nn.Module):
                         ops.flash_attn(q[rows], ki[:, :C], ki[:, C:], T, HW, ki.shape[0] // T, heads, out=a[rows], accumulate=True)
                     else:
                         ops.flash_attn(q[rows], ki[:, :C], ki[:, C:], T, HW, ki.shape[0], heads, kv_shared=True, out=a[rows], accumulate=True)
-            x = ops.linear(a, Q["o2_w"], bias=Q["o2_b"], res=x, ln_out=fold)
-            x, st = x if fold else (x, None)
-            g = _ln_linear(Q, x, "ff1", "ln3", st, geglu=True)
-            last = Q is P["blocks"][-1]
-            x = ops.linear(g, Q["ff2_w"], bias=Q["ff2_b"], res=x, ln_out=fold and not last)
-            x, st = x if (fold and not last) else (x, None)
+            x, st = ops.linear(a, Q["o2_w"], bias=Q["o2_b"], res=x, ln_out=True)
+            x, st = _ff(Q, x, st, Q is P["blocks"][-1])
         # out_plan (multi-GPU): proj_out's epilogue performs the frames -> sites switch the TemporalTransformer that follows needs
         return ops.linear(x, P["out_w"], bias=P["out_b"], res=h, gn_out=True, peer=out_plan)
 
@@ -529,22 +513,17 @@ class UNetModel(nn.Module):
         C = heads * 64
         Tg, HWl = (comm.T, HW // comm.world) if comm else (T, HW)
         t_in = h if pre_sites else (comm.to_sites(h, B, HW) if comm else h)
-        fold = _LN_FOLD
-        x = ops.linear(UNetModel._gn5d(t_in, B, *P["gn"], 1e-6, False, comm, Tg * HW, HW, fresh=True), P["in_w"], bias=P["in_b"], ln_out=fold)
-        x, st = x if fold else (x, None)
+        x, st = ops.linear(UNetModel._gn5d(t_in, B, *P["gn"], 1e-6, False, comm, Tg * HW, HW, fresh=True), P["in_w"], bias=P["in_b"],
+                           ln_out=True)
         for Q in P["blocks"]:
-            for ln, wqkv, ow, ob in (("ln1", "qkv1", "o1_w", "o1_b"), ("ln2", "qkv2", "o2_w", "o2_b")):
-                qkv = _ln_linear(Q, x, wqkv, ln, st)
+            for wqkv, ow, ob in (("qkv1", "o1_w", "o1_b"), ("qkv2", "o2_w", "o2_b")):
+                qkv = _ln_linear(Q, x, st, wqkv)
                 a = torch.empty((qkv.shape[0], C), device=qkv.device, dtype=torch.float16)
                 for b in range(B):
                     rows = slice(b * Tg * HWl, (b + 1) * Tg * HWl)
                     ops.temporal_attn(qkv[rows, :C], qkv[rows, C:2 * C], qkv[rows, 2 * C:], Tg, HWl, heads, out=a[rows])
-                x = ops.linear(a, Q[ow], bias=Q[ob], res=x, ln_out=fold)
-                x, st = x if fold else (x, None)
-            g = _ln_linear(Q, x, "ff1", "ln3", st, geglu=True)
-            last = Q is P["blocks"][-1]
-            x = ops.linear(g, Q["ff2_w"], bias=Q["ff2_b"], res=x, ln_out=fold and not last)
-            x, st = x if (fold and not last) else (x, None)
+                x, st = ops.linear(a, Q[ow], bias=Q[ob], res=x, ln_out=True)
+            x, st = _ff(Q, x, st, Q is P["blocks"][-1])
         to_f = comm.scatter_plan(False, B, HW, P["out_w"].shape[0]) if comm else None
         out = ops.linear(x, P["out_w"], bias=P["out_b"], res=t_in, gn_out=comm is None, peer=to_f)
         return out if to_f is not None else (comm.to_frames(out, B, HW) if comm else out)
