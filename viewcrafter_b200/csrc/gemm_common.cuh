@@ -1,5 +1,5 @@
-// Shared pieces of the tap-GEMM kernel (gemm_tap.cu): parameter block, tile enumeration and the per-chunk epilogue
-// (bias / folded LayerNorm / residual / statistics / store) that runs on one output row x 32 columns per thread.
+// Shared pieces of the tap-GEMM kernel (gemm_tap.cu): parameter block, tile enumeration, the shared-memory output tile and
+// the row passes of the epilogue over it (statistics, non-TMA stores, multi-GPU scatter).
 #pragma once
 #include "common.cuh"
 
@@ -17,14 +17,15 @@ static constexpr int GEMM_LAUNCH_REGS = 168;
 static constexpr int GEMM_PRODUCER_REGS = 24;
 static constexpr int GEMM_MMA_REGS = 240;
 static_assert(128 * GEMM_PRODUCER_REGS + 128 * MMA_WGS * GEMM_MMA_REGS <= GEMM_LAUNCH_REGS * GEMM_THREADS, "register split exceeds the CTA's allocation");
-static constexpr int EPI_WARPS = 4 * MMA_WGS;
-static constexpr int EPI_STAGE_BYTES = 32 * 32 * 2;              // one warp's staging tile for TMA stores: 32 rows x 32 fp16
-// accumulator transpose: an MMA warpgroup writes 64 rows x 64 columns of fp32 at a time, then each warp reads back 32 rows x
-// 32 columns with one row per thread.  Row pitch 72 floats: the fragment writes (8 rows x 4 column pairs per warp) hit 32
-// distinct banks per half warp.
-static constexpr int EPI_XPOSE_PITCH = 72;
-static constexpr int EPI_XPOSE_BYTES = 64 * EPI_XPOSE_PITCH * 4;
-static constexpr int EPI_SMEM_BYTES = EPI_WARPS * EPI_STAGE_BYTES + MMA_WGS * EPI_XPOSE_BYTES;
+// Output tile of an MMA warpgroup: 128 rows x BN fp16 columns in shared memory, one 8 KB block per 32-column chunk, each
+// block 128 rows of 64 bytes with the 64B swizzle (16-byte unit u of row R stored at unit u ^ ((R >> 1) & 3)).  Rows 32 q ..
+// 32 q + 31 of a chunk form the 2 KB box the TMA stores write (tmap_out, peer maps); a whole 8 KB block is the box of a
+// residual load (tmap_res).
+static constexpr int EPI_CHUNK_BYTES = BM * 32 * 2;
+static constexpr int EPI_SUB_BYTES = 32 * 32 * 2;
+__host__ __device__ constexpr uint32_t epi_offset(int row, int col) {   // byte offset of element (row, col) in the output tile
+  return (uint32_t)((col >> 5) * EPI_CHUNK_BYTES + row * 64 + ((((col & 31) >> 3) ^ ((row >> 1) & 3)) << 4) + (col & 7) * 2);
+}
 
 // Division by a runtime constant as multiply-high + shift (valid for dividends < 2^31): the persistent kernels turn a
 // linear tile index into (n-tile, x, y, z) once per tile in EVERY thread, and a generic 32-bit division is ~20 SASS
@@ -71,6 +72,7 @@ struct GemmParams {
   CUtensorMap tmap_a2;
   CUtensorMap tmap_b;
   CUtensorMap tmap_out;  // fp16 output as (N, X, Y, Z), box (32, min(bx,32), 32/min(bx,32), 1), 64B swizzle (out_tma only)
+  CUtensorMap tmap_res;  // residual as (N, X, Y, Z), box (32, bx, by, 1), 64B swizzle (res_tma only)
   int tiles_x, tiles_y, Z;
   FastDiv div_tiles_x, div_tiles_y, div_n_tiles;
   int bx, by;
@@ -97,9 +99,9 @@ struct GemmParams {
   float2* gn_part;         // optional: GroupNorm partial (sum, sumsq) of the fp16-rounded outputs per (32-row block, 32-column chunk, piece):
   int gn_hp;               //   [m_tile * 4 + quadrant][N / 32][4]; a chunk is cut at the boundaries of gn_sub = 2 * gn_hp channel sub-groups
   int gn_nchunks;          //   (4 pieces: first partial, two whole, last partial / whole) -- see gn_part_accumulate and norm.cu: gn_part_finalize_kernel
-  int out_tma;           // fp16 output written by TMA stores from per-warp staging tiles (full-line, LSU-free)
-  int vec_ok;            // output rows are 32-byte aligned: whole 32-column chunks of a non-TMA output are stored as 256-bit vectors
-  int res_vec;           // residual rows are 32-byte aligned: whole 32-column chunks of the residual are loaded as 256-bit vectors
+  int out_tma;           // fp16 output written by TMA stores from the warpgroup's output tile (full-line, LSU-free)
+  int vec_ok;            // output rows are 32-byte aligned: a non-TMA output is stored as 256-bit (fp16) / 64-bit (fp32) vectors
+  int res_tma;           // residual 16-byte aligned with a 16-byte row pitch: loaded by TMA into the output tile while the MMAs run
   GemmPeer peer;         // output scattered to the ranks of the frame group (mode != 0: `out` itself is not written)
   // FP8 mode (gemm_tap_kernel<BN, true>): e4m3 weights, A converted to e4m3 in registers with the per-tensor scale
   // s_a = a_amax / 448; the epilogue starts from acc * (s_a * w_scale[n])
@@ -144,12 +146,11 @@ __device__ __forceinline__ float gelu_epilogue(float x) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Epilogue chunk: one thread owns one output row and 32 consecutive columns (the accumulator was transposed through shared
-// memory by gemm_tap_kernel), a warp owns 32 consecutive rows of the tile: quad = 32-row block of the 128-row tile.
+// Row passes over the fp16 output tile (statistics, non-TMA stores): one thread owns one output row and the 32 columns of a
+// chunk, a warp owns 32 consecutive rows of the tile: quad = 32-row block of the 128-row tile.
 // ---------------------------------------------------------------------------------------------------------------
 struct EpiTile {
   long long orow;        // output row index of this thread
-  const float* bias;     // bias row for this tile's z (or nullptr)
   int n_tile;
   int m_tile;            // linear m-tile index (x fastest, then y, then z)
   int quad;              // 32-row block of the tile owned by this warp
@@ -170,11 +171,10 @@ __device__ __forceinline__ EpiTile epi_tile(const GemmParams& p, int tile, int q
   const int x = tc.x0 + (R & (p.bx - 1)), y = tc.y0 + (R >> p.bx_shift);
   t.row_ok = x < p.X && y < p.Y && tc.z < p.Z;
   t.orow = ((long long)tc.z * p.Y + y) * p.X + x;
-  t.bias = p.bias ? p.bias + (long long)(p.bias_z_div > 0 ? min(tc.z, p.Z - 1) / p.bias_z_div : 0) * p.N : nullptr;
   return t;
 }
 
-// peer mode: the warp's staged 32 x 32 tile goes to the rank(s) owning its rows in the other layout (executed by one lane)
+// peer mode: the warp's 32 x 32 box of the output tile goes to the rank(s) owning its rows in the other layout (executed by one lane)
 __device__ __forceinline__ void peer_scatter32(const GemmParams& p, const EpiTile& t, int col0, const uint8_t* stage) {
   const GemmPeer& g = p.peer;
   int lin = t.wy * p.X + t.wx;                 // first row of the warp's patch inside its z-slab (patches are row-contiguous: host check)
@@ -203,56 +203,28 @@ __device__ __forceinline__ void peer_scatter32(const GemmParams& p, const EpiTil
   }
 }
 
-// store 32 consecutive output columns of this thread's row (fp16 or fp32): TMA store, vector path or predicated scalar path.
-// f holds the final values (bias and residual already added by epi_chunk): every path rounds the same fp32 values once,
-// round-to-nearest, so the fp16 output does not depend on which path its pointer and pitch select.
-__device__ __forceinline__ void epi_store32(const GemmParams& p, const EpiTile& t, int col0, int n_out, float (&f)[32],
-                                            uint8_t* stage, int lane) {
-  if (p.out_tma) {
-    // Stage the warp's 32 x 32 fp16 tile in shared memory (64B-swizzled rows: conflict-free 16-byte stores) and let the TMA
-    // unit write it: rows outside (X, Y, Z) are clipped by the tensor map.  Row-per-thread global stores would touch 32
-    // different 128-byte lines per instruction.
-    if (lane == 0) tma_store_wait_read();          // the previous store has finished reading this warp's staging tile
-    __syncwarp();
-    const uint32_t sbase = smem_u32(stage) + lane * 64;
-    const int sw = (lane >> 1) & 3;
+// the 32 fp16 values of this thread's row in one chunk of the output tile (row_addr: shared address of the row), in column order
+__device__ __forceinline__ void epi_row_load(uint32_t row_addr, int row, uint4 (&u)[4]) {
+  const int sw = (row >> 1) & 3;
 #pragma unroll
-    for (int h = 0; h < 4; ++h) {
-      const uint32_t u0 = pack_half2(f[h * 8 + 0], f[h * 8 + 1]), u1 = pack_half2(f[h * 8 + 2], f[h * 8 + 3]);
-      const uint32_t u2 = pack_half2(f[h * 8 + 4], f[h * 8 + 5]), u3 = pack_half2(f[h * 8 + 6], f[h * 8 + 7]);
-      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sbase + ((h ^ sw) << 4)), "r"(u0), "r"(u1), "r"(u2), "r"(u3) : "memory");
-    }
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) {
-      if (p.peer.mode) peer_scatter32(p, t, col0, stage);
-      else tma_store_4d(&p.tmap_out, stage, col0, t.wx, t.wy, t.wz);
-      tma_store_commit();
-    }
-    return;
-  }
+  for (int h = 0; h < 4; ++h)
+    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(u[h].x), "=r"(u[h].y), "=r"(u[h].z), "=r"(u[h].w) : "r"(row_addr + ((h ^ sw) << 4)));
+}
+
+// fp16 output that the TMA store cannot write (unaligned pointer or pitch, ragged N): this thread's row of one chunk, copied
+// from the output tile as 256-bit vectors, or by predicated scalar stores at a ragged N tail / unaligned pitch (the 320->4
+// output conv).  The values were rounded once in the tile, so the output does not depend on the store path.
+__device__ __forceinline__ void epi_store_row32(const GemmParams& p, const EpiTile& t, int col0, int n_out, const uint4 (&u)[4]) {
   if (!t.row_ok || col0 >= n_out) return;
   if (col0 + 32 <= n_out && p.vec_ok) {
-    if (p.out_f32) {
-      float4* op = reinterpret_cast<float4*>(p.out_f32 + t.orow * p.ldo + col0);
+    uint4* op = reinterpret_cast<uint4*>(p.out + t.orow * p.ldo + col0);
 #pragma unroll
-      for (int h = 0; h < 8; ++h) op[h] = make_float4(f[h * 4], f[h * 4 + 1], f[h * 4 + 2], f[h * 4 + 3]);
-    } else {
-      uint4* op = reinterpret_cast<uint4*>(p.out + t.orow * p.ldo + col0);
-#pragma unroll
-      for (int h = 0; h < 4; ++h)
-        op[h] = make_uint4(pack_half2(f[h * 8 + 0], f[h * 8 + 1]), pack_half2(f[h * 8 + 2], f[h * 8 + 3]), pack_half2(f[h * 8 + 4], f[h * 8 + 5]),
-                           pack_half2(f[h * 8 + 6], f[h * 8 + 7]));
-    }
+    for (int h = 0; h < 4; ++h) op[h] = u[h];
   } else {
-    // ragged N tail / unaligned pitch (e.g. the 320->4 output conv): predicated scalar path
+    const __half* hv = reinterpret_cast<const __half*>(u);
 #pragma unroll
-    for (int e = 0; e < 32; ++e) {
-      if (col0 + e < n_out) {
-        if (p.out_f32) p.out_f32[t.orow * p.ldo + col0 + e] = f[e];
-        else p.out[t.orow * p.ldo + col0 + e] = __float2half_rn(f[e]);
-      }
-    }
+    for (int e = 0; e < 32; ++e)
+      if (col0 + e < n_out) p.out[t.orow * p.ldo + col0 + e] = hv[e];
   }
 }
 
@@ -332,88 +304,26 @@ __device__ __forceinline__ void gn_part_accumulate(const GemmParams& p, const Ep
   }
 }
 
-// FP8 dequantisation of one 32-column chunk: f = acc * (s_a * w_scale[n]), in fp32
-__device__ __forceinline__ void fp8_dequant32(const GemmParams& p, int nb, float sa, float (&f)[32]) {
-  if (nb + 32 <= p.N) {
+// LayerNorm / GroupNorm statistics of this thread's row of one 32-column chunk (nb: its first column), from the fp16 values
+// the output holds (u: epi_row_load)
+__device__ __forceinline__ void epi_stats_row32(const GemmParams& p, const EpiTile& t, int nb, const uint4 (&u)[4], int lane) {
+  float f[32];
+  const __half2* h2 = reinterpret_cast<const __half2*>(u);
 #pragma unroll
-    for (int e = 0; e < 32; e += 4) {
-      const float4 w4 = __ldg(reinterpret_cast<const float4*>(p.w_scale + nb + e));
-      f[e] *= sa * w4.x; f[e + 1] *= sa * w4.y; f[e + 2] *= sa * w4.z; f[e + 3] *= sa * w4.w;
-    }
-  } else {
-#pragma unroll
-    for (int e = 0; e < 32; ++e)
-      if (nb + e < p.N) f[e] *= sa * __ldg(p.w_scale + nb + e);
+  for (int e = 0; e < 16; ++e) {
+    const float2 r = __half22float2(h2[e]);
+    f[2 * e] = r.x; f[2 * e + 1] = r.y;
   }
-}
-
-// One 32-column chunk of this thread's row: folded LayerNorm, bias, residual, output statistics, store.
-// nb: first column in the accumulator's N space (bias / LayerNorm column sums / residual / statistics), col0: first output column.
-// plain: the values are final already (GEGLU, computed on the fragments), only statistics-free storing remains.
-// The residual is added here, in registers, whatever the store path: the statistics and every store path see the same values.
-// FP8: f holds the raw e4m3 products' sums; they are dequantised with the activation scale sa first, then the fp16 epilogue runs.
-template <bool FP8 = false>
-__device__ __forceinline__ void epi_chunk(const GemmParams& p, const EpiTile& t, int nb, int col0, int n_out, bool plain, float (&f)[32],
-                                          uint8_t* stage, int lane, float sa = 1.f) {
-  if (!plain) {
-    if constexpr (FP8) fp8_dequant32(p, nb, sa, f);
-    if (p.ln_stats) {                              // folded LayerNorm (host guarantees N % 32 == 0)
-      const float2 ln = t.row_ok ? __ldg(reinterpret_cast<const float2*>(p.ln_stats) + t.orow) : make_float2(0.f, 1.f);
+  if (p.ln_part) {                                 // LayerNorm statistics of the OUTPUT row, as stored (fp16-rounded)
+    float s = 0.f, q = 0.f;
 #pragma unroll
-      for (int e = 0; e < 32; e += 4) {
-        const float4 cs = __ldg(reinterpret_cast<const float4*>(p.ln_colsum + nb + e));
-        f[e] = (f[e] - ln.x * cs.x) * ln.y; f[e + 1] = (f[e + 1] - ln.x * cs.y) * ln.y;
-        f[e + 2] = (f[e + 2] - ln.x * cs.z) * ln.y; f[e + 3] = (f[e + 3] - ln.x * cs.w) * ln.y;
-      }
+    for (int e = 0; e < 32; e += 2) {
+      s += f[e] + f[e + 1];
+      q = fmaf(f[e], f[e], fmaf(f[e + 1], f[e + 1], q));
     }
-    if (t.bias) {
-      if (nb + 32 <= p.N) {
-#pragma unroll
-        for (int e = 0; e < 32; e += 4) {
-          const float4 b4 = __ldg(reinterpret_cast<const float4*>(t.bias + nb + e));
-          f[e] += b4.x; f[e + 1] += b4.y; f[e + 2] += b4.z; f[e + 3] += b4.w;
-        }
-      } else {
-#pragma unroll
-        for (int e = 0; e < 32; ++e)
-          if (nb + e < p.N) f[e] += __ldg(t.bias + nb + e);
-      }
-    }
-    // plain loads, not __ldg: res may alias out (in-place residual)
-    if (p.res != nullptr && t.row_ok) {
-      if (p.res_vec && nb + 32 <= p.N) {
-        const uint4* rp = reinterpret_cast<const uint4*>(p.res + t.orow * p.ldr + nb);
-#pragma unroll
-        for (int h = 0; h < 4; ++h) {
-          const uint4 u = rp[h];
-          const __half2* r2 = reinterpret_cast<const __half2*>(&u);
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float2 r = __half22float2(r2[e]);
-            f[h * 8 + 2 * e] += r.x; f[h * 8 + 2 * e + 1] += r.y;
-          }
-        }
-      } else {
-        // ragged N tail / residual rows not 32-byte aligned: predicated scalar loads
-        const __half* rp = p.res + t.orow * p.ldr + nb;
-#pragma unroll
-        for (int e = 0; e < 32; ++e)
-          if (nb + e < p.N) f[e] += __half2float(rp[e]);
-      }
-    }
-    if (p.ln_part) {                               // LayerNorm statistics of the OUTPUT row, as stored (fp16-rounded)
-      float s = 0.f, q = 0.f;
-#pragma unroll
-      for (int e = 0; e < 32; e += 2) {
-        const float2 r = __half22float2(__floats2half2_rn(f[e], f[e + 1]));
-        s += r.x + r.y;
-        q = fmaf(r.x, r.x, fmaf(r.y, r.y, q));
-      }
-      if (t.row_ok) p.ln_part[(long long)(nb >> 5) * p.ln_rows + t.orow] = make_float2(s, q);
-    }
-    if (p.gn_part) gn_part_accumulate(p, t, nb, f, lane);
+    if (t.row_ok) p.ln_part[(long long)(nb >> 5) * p.ln_rows + t.orow] = make_float2(s, q);
   }
-  epi_store32(p, t, col0, n_out, f, stage, lane);
+  if (p.gn_part) gn_part_accumulate(p, t, nb, f, lane);
 }
 #endif  // __CUDACC__
 

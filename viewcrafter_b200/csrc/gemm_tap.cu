@@ -6,7 +6,8 @@
 //                                       the zero padding is TMA out-of-bounds fill
 //   * Conv3d (3,1,1), pad (1,0,0)     : 3 taps, A rows shifted by +-H*W rows of the [T*H*W, C] matrix (OOB rows = 0)
 // A may come from two tensors split along K (channel concat of skip connections without materialising it).
-// Epilogue: + bias[z/bias_z_div][n], GEGLU (value*gelu(gate)), + residual, fp16 / fp32 store (gemm_common.cuh).
+// Epilogue (epi_tile_run): + bias[z/bias_z_div][n], GEGLU (value*gelu(gate)), + residual, fp16 / fp32 store, on the accumulator
+// fragments; fp16 results go through a shared-memory output tile that the TMA stores (and the statistics) read.
 //
 // Persistent kernel, one CTA per SM, 128 x BN tiles, 384 threads, ping-pong schedule:
 //   warpgroup 0  warp 0 is the TMA producer: it walks this CTA's tiles and their (tap, k-block) iterations through a smem
@@ -16,7 +17,8 @@
 //                whole 128 x BN tile as two wgmma m64nBNk16 row halves (both operands from the 128B-swizzled ring, one k-block
 //                in flight behind the one being issued), consumes only its own tiles' ring stages, and steps its ring
 //                position past the other warpgroup's.  Then it runs the epilogue of its tile while the other warpgroup's
-//                MMAs keep the tensor cores busy.
+//                MMAs keep the tensor cores busy.  A tile's residual is TMA-loaded into the warpgroup's output tile when
+//                its mainloop starts, so the epilogue finds it in shared memory.
 //   The mainloops alternate strictly (an ordering barrier between the two MMA warpgroups): a warpgroup starts waiting on its
 //   next tile's stages only once the other one has seen all of its own.  Besides keeping the two mainloops from sharing the
 //   tensor cores, this keeps every full-barrier wait within one phase of the barrier, which the parity waits require.
@@ -29,6 +31,8 @@
 // HBM: no conversion pass.  The epilogue starts from acc * (s_a * w_scale[n]) and is otherwise the fp16 one.
 #include <cuda_fp8.h>
 
+#include <type_traits>
+
 #include "gemm_common.cuh"
 #include "kernels.h"
 #include "wgmma.cuh"
@@ -40,45 +44,182 @@ struct GemmCfg {
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * (FP8 ? 1 : 2);
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int BUDGET = 227 * 1024 - 1024 /*align slack*/ - 256 /*barriers*/ - EPI_SMEM_BYTES;
+  static constexpr int OUT_BYTES = BM * BN * 2;        // one MMA warpgroup's fp16 output tile (gemm_common.cuh: epi_offset)
+  static constexpr int EPI_BYTES = MMA_WGS * OUT_BYTES;
+  static constexpr int BUDGET = 227 * 1024 - 1024 /*align slack*/ - 256 /*barriers*/ - EPI_BYTES;
   static constexpr int STAGES = BUDGET / STAGE_BYTES > 8 ? 8 : BUDGET / STAGE_BYTES;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_SMEM_BYTES + 1024 + 256;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + 1024 + 256;
   static_assert(STAGES >= 4, "pipeline too shallow");
   static_assert(B_BYTES % 1024 == 0, "stages must stay 1024-byte aligned (128B swizzle atoms)");
+  static_assert(BN % 32 == 0, "the output tile is made of 32-column chunks");
 };
 
-// Drain the accumulator fragments of one 64-row half of an MMA warpgroup's tile (64 rows x NCOLS columns) through the
-// warpgroup's transpose buffer, 64 columns at a time, and run the per-chunk epilogue with one row per thread: warp wl of the
-// warpgroup takes rows (wl & 1) * 32 + lane of the half and chunk (wl >> 1) of each 64-column slab.
-template <int BN, int NCOLS, bool FP8 = false>
-__device__ __forceinline__ void epi_drain(const GemmParams& p, const EpiTile& t, float (&acc)[BN / 2], float* xpose, int cw, int wl, int lane,
-                                          uint8_t* stage, bool plain, int nb0, int col0, int n_out, float sa = 1.f) {
-  constexpr int SLABS = (NCOLS + 63) / 64;
-  const int fr = 16 * wl + (lane >> 2), fc = 2 * (lane & 3);   // fragment row / column of d[j * 4] (wgmma accumulator layout)
+// bias / LayerNorm column sums / weight scales of columns n and n + 1 (n even, the vectors 8-byte aligned); 0 past N
+__device__ __forceinline__ float2 col_pair(const float* v, int n, int N) {
+  if (n + 1 < N) return __ldg(reinterpret_cast<const float2*>(v + n));
+  return make_float2(n < N ? __ldg(v + n) : 0.f, 0.f);
+}
+
+// Epilogue of one 128 x BN tile, run by the MMA warpgroup that computed it, on its accumulator fragments.  Thread (warp wl,
+// lane) holds rows R = 64 h + 16 wl + lane / 4 + 8 r and columns c = 8 j + 2 (lane % 4) + {0, 1} of the tile in
+// acc[h][4 j + 2 r + {0, 1}].  Per element, in this order: FP8 dequantisation, folded LayerNorm, bias, residual, one rounding
+// to fp16 -- or, for GEGLU, value * gelu(gate) of the column pair (c, c + BN / 2).  The residual comes from the output tile,
+// where the TMA load issued at the start of the tile's mainloop left it, at the element's own position, and the fp16 result
+// goes back to the same position (one owner per element: no barrier).  fp32 outputs are stored straight from the fragments.
+// After one warpgroup barrier, warp wl takes rows 32 wl .. 32 wl + 31 of the tile: the statistics and the non-TMA stores read
+// them one row per thread, and lane 0 issues the TMA stores of the warp's 32 x 32 boxes.
+template <int BN, bool FP8>
+__device__ __forceinline__ void epi_tile_run(const GemmParams& p, int tile, float (&acc)[2][BN / 2], uint8_t* otile,
+                                             uint64_t* res_bar, int cw, int wl, int lane, float sa) {
+  const int m_tile = fast_div(p.div_n_tiles, tile);
+  const int n_tile = tile - m_tile * p.n_tiles;
+  const TileCoord tc = tile_coord_m(p, m_tile);
+  const int n0 = n_tile * BN;
+  const bool geglu = BN == 128 && p.geglu;         // GEGLU always runs at BN = 128 (pick_bn)
+  const int n_out = geglu ? p.N / 2 : p.N;
+  const int col_base = geglu ? n_tile * (BN / 2) : n0;
+  const float* bias = p.bias ? p.bias + (long long)(p.bias_z_div > 0 ? min(tc.z, p.Z - 1) / p.bias_z_div : 0) * p.N : nullptr;
+  const uint32_t obase = smem_u32(otile);
+  const int q = lane & 3;
+  bool row_ok[2][2];
+  long long orow[2][2];
+  float2 ln[2][2];
 #pragma unroll
-  for (int sl = 0; sl < SLABS; ++sl) {
-    named_bar_sync(1 + cw, 128);                   // the previous slab has been read back
+  for (int h = 0; h < 2; ++h)
 #pragma unroll
-    for (int jj = 0; jj < 8; ++jj) {
-      const int j = sl * 8 + jj;
-      if (j < NCOLS / 8) {
-        float* d0 = xpose + fr * EPI_XPOSE_PITCH + jj * 8 + fc;
-        *reinterpret_cast<float2*>(d0) = make_float2(acc[j * 4], acc[j * 4 + 1]);
-        *reinterpret_cast<float2*>(d0 + 8 * EPI_XPOSE_PITCH) = make_float2(acc[j * 4 + 2], acc[j * 4 + 3]);
+    for (int r = 0; r < 2; ++r) {
+      const int R = 64 * h + 16 * wl + (lane >> 2) + 8 * r;
+      const int x = tc.x0 + (R & (p.bx - 1)), y = tc.y0 + (R >> p.bx_shift);
+      row_ok[h][r] = x < p.X && y < p.Y && tc.z < p.Z;
+      orow[h][r] = ((long long)tc.z * p.Y + y) * p.X + x;
+      ln[h][r] = make_float2(0.f, 1.f);
+      if (p.ln_stats && row_ok[h][r]) ln[h][r] = __ldg(reinterpret_cast<const float2*>(p.ln_stats) + orow[h][r]);
+    }
+  const bool res_smem = p.res && p.res_tma;
+  // tile = blockIdx.x + cw * gridDim.x + 2 * gridDim.x * k: the k-th residual load of this warpgroup completes phase k & 1
+  if (res_smem) mbar_wait(res_bar, ((tile - (int)blockIdx.x) / (2 * (int)gridDim.x)) & 1);
+  // The common case (fp16 output, residual from the tile or none) runs a loop without per-element branches on the store path:
+  // those branches cost the loop its scheduling and made it several times slower.  fp32 outputs and residuals TMA cannot load
+  // take the general loop.
+  auto frag_loop = [&](auto general_tag) {
+    constexpr bool GENERAL = decltype(general_tag)::value;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int c = 8 * j + 2 * q;
+      const int n = n0 + c;
+      float2 ws = make_float2(1.f, 1.f), cs = make_float2(0.f, 0.f), b = make_float2(0.f, 0.f);
+      if constexpr (FP8) ws = col_pair(p.w_scale, n, p.N);
+      if (p.ln_stats) cs = col_pair(p.ln_colsum, n, p.N);
+      if (bias) b = col_pair(bias, n, p.N);
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const int R = 64 * h + 16 * wl + (lane >> 2) + 8 * r;
+          const uint32_t addr = obase + epi_offset(R, c);
+          float v0 = acc[h][4 * j + 2 * r], v1 = acc[h][4 * j + 2 * r + 1];
+          if constexpr (FP8) { v0 *= sa * ws.x; v1 *= sa * ws.y; }
+          if (p.ln_stats) {
+            const float2 l = ln[h][r];
+            v0 = (v0 - l.x * cs.x) * l.y;
+            v1 = (v1 - l.x * cs.y) * l.y;
+          }
+          if (bias) { v0 += b.x; v1 += b.y; }
+          if (res_smem) {
+            uint32_t u;
+            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(u) : "r"(addr));
+            const float2 rv = __half22float2(*reinterpret_cast<const __half2*>(&u));
+            v0 += rv.x; v1 += rv.y;
+          } else if (GENERAL && p.res && row_ok[h][r]) {
+            // residual TMA cannot address (unaligned pointer or pitch): plain loads, not __ldg -- res may alias out
+            const __half* rp = p.res + orow[h][r] * p.ldr + n;
+            if (n < p.N) v0 += __half2float(rp[0]);
+            if (n + 1 < p.N) v1 += __half2float(rp[1]);
+          }
+          if (GENERAL && p.out_f32) {
+            if (row_ok[h][r] && n < n_out) {
+              float* op = p.out_f32 + orow[h][r] * p.ldo + n;
+              if (n + 1 < n_out && p.vec_ok) {
+                *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
+              } else {
+                op[0] = v0;
+                if (n + 1 < n_out) op[1] = v1;
+              }
+            }
+          } else {
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_half2(v0, v1)) : "memory");
+          }
+        }
+    }
+  };
+  if (!geglu) {
+    if (p.out_f32 || (p.res && !p.res_tma)) frag_loop(std::true_type{});
+    else frag_loop(std::false_type{});
+  } else {
+    // GEGLU: tile columns [0, BN/2) are values, [BN/2, BN) the matching gates (weights were interleaved per tile);
+    // out[:, n_tile*BN/2 + c] = (value + bias_v) * gelu(gate + bias_g).  No residual (checked on the host).
+    constexpr int HALF = BN / 2;
+#pragma unroll
+    for (int j = 0; j < HALF / 8; ++j) {
+      const int c = 8 * j + 2 * q;
+      const int n = n0 + c;
+      float2 wv = make_float2(1.f, 1.f), wg = wv, cv = make_float2(0.f, 0.f), cg = cv, bv = cv, bg = cv;
+      if constexpr (FP8) { wv = col_pair(p.w_scale, n, p.N); wg = col_pair(p.w_scale, n + HALF, p.N); }
+      if (p.ln_stats) { cv = col_pair(p.ln_colsum, n, p.N); cg = col_pair(p.ln_colsum, n + HALF, p.N); }
+      if (bias) { bv = col_pair(bias, n, p.N); bg = col_pair(bias, n + HALF, p.N); }
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const int R = 64 * h + 16 * wl + (lane >> 2) + 8 * r;
+          float o[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            float a = acc[h][4 * j + 2 * r + e], g = acc[h][4 * (j + HALF / 8) + 2 * r + e];
+            if constexpr (FP8) {
+              a *= sa * (e ? wv.y : wv.x);
+              g *= sa * (e ? wg.y : wg.x);
+            }
+            if (p.ln_stats) {
+              const float2 l = ln[h][r];
+              a = (a - l.x * (e ? cv.y : cv.x)) * l.y;
+              g = (g - l.x * (e ? cg.y : cg.x)) * l.y;
+            }
+            if (bias) { a += e ? bv.y : bv.x; g += e ? bg.y : bg.x; }
+            o[e] = a * gelu_epilogue(g);
+          }
+          asm volatile("st.shared.b32 [%0], %1;" ::"r"(obase + epi_offset(R, c)), "r"(pack_half2(o[0], o[1])) : "memory");
+        }
+    }
+  }
+  if (p.out_f32) return;                           // no statistics on fp32 outputs (host check)
+  if (p.out_tma) fence_proxy_async_smem();         // the fp16 tile is visible to the TMA stores
+  named_bar_sync(1 + cw, 128);
+  constexpr int CHUNKS = BN / 32;
+  const int nchunks = geglu ? CHUNKS / 2 : CHUNKS;
+  const EpiTile t = epi_tile(p, tile, wl, lane);
+  if (p.ln_part || p.gn_part || !p.out_tma) {
+    const int R = 32 * wl + lane;
+#pragma unroll
+    for (int c = 0; c < CHUNKS; ++c) {
+      if (c < nchunks && col_base + 32 * c < n_out) {   // warp-uniform
+        uint4 u[4];
+        epi_row_load(obase + c * EPI_CHUNK_BYTES + R * 64, R, u);
+        if (p.ln_part || p.gn_part) epi_stats_row32(p, t, n0 + 32 * c, u, lane);
+        if (!p.out_tma) epi_store_row32(p, t, col_base + 32 * c, n_out, u);
       }
     }
-    named_bar_sync(1 + cw, 128);
-    const int c = sl * 2 + (wl >> 1);
-    if (c * 32 < NCOLS && (plain ? col0 + c * 32 < n_out : nb0 + c * 32 < p.N)) {   // warp-uniform
-      float f[32];
-      const float4* src = reinterpret_cast<const float4*>(xpose + ((wl & 1) * 32 + lane) * EPI_XPOSE_PITCH + (wl >> 1) * 32);
+  }
+  if (p.out_tma && lane == 0) {
 #pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        const float4 v = src[e];
-        f[4 * e] = v.x; f[4 * e + 1] = v.y; f[4 * e + 2] = v.z; f[4 * e + 3] = v.w;
+    for (int c = 0; c < CHUNKS; ++c) {
+      if (c < nchunks && col_base + 32 * c < n_out) {
+        const uint8_t* box = otile + c * EPI_CHUNK_BYTES + wl * EPI_SUB_BYTES;
+        if (p.peer.mode) peer_scatter32(p, t, col_base + 32 * c, box);
+        else tma_store_4d(&p.tmap_out, box, col_base + 32 * c, t.wx, t.wy, t.wz);
       }
-      epi_chunk<FP8>(p, t, nb0 + c * 32, col0 + c * 32, n_out, plain, f, stage, lane, sa);
     }
+    tma_store_commit();
   }
 }
 
@@ -100,9 +241,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tap_kernel(const __grid_
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* epi_smem = smem + STAGES * Cfg::STAGE_BYTES;          // [EPI_WARPS] TMA-store staging tiles, [MMA_WGS] transpose buffers
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi_smem + EPI_SMEM_BYTES);
+  uint8_t* epi_smem = smem + STAGES * Cfg::STAGE_BYTES;          // [MMA_WGS] output tiles
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi_smem + Cfg::EPI_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* res_bar = empty_bar + STAGES;                         // [MMA_WGS] residual loaded into the output tile
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -113,10 +255,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tap_kernel(const __grid_
     tma_prefetch_desc(&p.tmap_a);
     tma_prefetch_desc(&p.tmap_b);
     if (p.out_tma) tma_prefetch_desc(&p.tmap_out);
+    if (p.res_tma) tma_prefetch_desc(&p.tmap_res);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 4);                  // one arrival per warp of the MMA warpgroup that owns the stage's tile
     }
+    for (int w = 0; w < MMA_WGS; ++w) mbar_init(&res_bar[w], 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -159,8 +303,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tap_kernel(const __grid_
     setmaxnreg_inc<GEMM_MMA_REGS>();
     const int cw = (warp >> 2) - 1;                 // tiles cw, cw + 2, cw + 4, ... of this CTA's sequence
     const int wl = warp & 3;
-    uint8_t* stage = epi_smem + (warp - 4) * EPI_STAGE_BYTES;
-    float* xpose = reinterpret_cast<float*>(epi_smem + EPI_WARPS * EPI_STAGE_BYTES + cw * EPI_XPOSE_BYTES);
+    uint8_t* otile = epi_smem + cw * Cfg::OUT_BYTES;
     const uint32_t ring = smem_u32(smem);
     float sa = 1.f, inv_sa = 1.f;                   // FP8: per-tensor activation scale s_a = amax / 448 (1 for an all-zero A)
     if constexpr (FP8) {
@@ -183,8 +326,22 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tap_kernel(const __grid_
     };
     if (cw == 1) skip_tile();
     for (int tile = blockIdx.x + cw * gridDim.x; tile < p.total_tiles; tile += 2 * gridDim.x) {
-      // ordering barrier: the other warpgroup has waited on every stage of the tile before this one (ids 3 / 4: "cw may start")
+      // this warpgroup's previous tile: its TMA stores have finished reading the output tile (each warp's lane 0 issued its own)
+      if (p.out_tma && lane == 0) tma_store_wait_read();
+      __syncwarp();
+      // ordering barrier: the other warpgroup has waited on every stage of the tile before this one (ids 3 / 4: "cw may start").
+      // It also waits for all of this warpgroup's threads, so the previous tile's epilogue is done with the output tile.
       if (tile >= (int)gridDim.x) named_bar_sync(3 + cw, 256);
+      if (p.res_tma && wl == 0 && lane == 0) {
+        // residual of this tile into the output tile: it lands while the mainloop runs (rows / columns outside the tensor read as 0)
+        const int m_tile = fast_div(p.div_n_tiles, tile);
+        const TileCoord tc = tile_coord_m(p, m_tile);
+        const int n0 = (tile - m_tile * p.n_tiles) * BN;
+        const int nch = min(BN, p.N - n0 + 31) / 32;
+        mbar_expect_tx(&res_bar[cw], nch * EPI_CHUNK_BYTES);
+        for (int c = 0; c < nch; ++c) tma_load_4d(otile + c * EPI_CHUNK_BYTES, &p.tmap_res, &res_bar[cw], n0 + 32 * c, tc.x0, tc.y0, tc.z);
+      }
+      __syncwarp();
       int prev = -1;
       for (int i = 0; i < iters; ++i) {
         mbar_wait(&full_bar[s], ph);
@@ -246,49 +403,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tap_kernel(const __grid_
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty_bar[prev]);
       }
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const EpiTile t = epi_tile(p, tile, h * 2 + (wl & 1), lane);
-        const int n0 = t.n_tile * BN;
-        if (BN != 128 || !p.geglu) {                   // GEGLU always runs at BN = 128 (pick_bn)
-          epi_drain<BN, BN, FP8>(p, t, acc[h], xpose, cw, wl, lane, stage, false, n0, n0, p.N, sa);
-        } else {
-          // GEGLU on the fragments: tile columns [0, BN/2) are values, [BN/2, BN) the matching gates (weights were interleaved
-          // per tile); out[:, n_tile*BN/2 + c] = (value + bias_v) * gelu(gate + bias_g).  No residual (checked on the host).
-          constexpr int HALF = BN / 2;
-          const TileCoord tc = tile_coord_m(p, t.m_tile);
-          float2 ln[2] = {make_float2(0.f, 1.f), make_float2(0.f, 1.f)};
-          if (p.ln_stats) {
-#pragma unroll
-            for (int r = 0; r < 2; ++r) {
-              const int R = h * 64 + 16 * wl + (lane >> 2) + 8 * r;
-              const int x = tc.x0 + (R & (p.bx - 1)), y = tc.y0 + (R >> p.bx_shift);
-              if (x < p.X && y < p.Y && tc.z < p.Z)
-                ln[r] = __ldg(reinterpret_cast<const float2*>(p.ln_stats) + ((long long)tc.z * p.Y + y) * p.X + x);
-            }
-          }
-#pragma unroll
-          for (int j = 0; j < HALF / 8; ++j) {
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const int n = n0 + 8 * j + 2 * (lane & 3) + (e & 1);
-              float a = acc[h][j * 4 + e], g = acc[h][(j + HALF / 8) * 4 + e];
-              if constexpr (FP8) {
-                a *= sa * __ldg(p.w_scale + n);
-                g *= sa * __ldg(p.w_scale + n + HALF);
-              }
-              if (p.ln_stats) {
-                const float2 l = ln[e >> 1];
-                a = (a - l.x * __ldg(p.ln_colsum + n)) * l.y;
-                g = (g - l.x * __ldg(p.ln_colsum + n + HALF)) * l.y;
-              }
-              if (t.bias) { a += __ldg(t.bias + n); g += __ldg(t.bias + n + HALF); }
-              acc[h][j * 4 + e] = a * gelu_epilogue(g);
-            }
-          }
-          epi_drain<BN, HALF>(p, t, acc[h], xpose, cw, wl, lane, stage, true, n0, t.n_tile * HALF, p.N / 2);
-        }
-      }
+      epi_tile_run<BN, FP8>(p, tile, acc, otile, &res_bar[cw], cw, wl, lane, sa);
     }
     if (p.out_tma && lane == 0) tma_store_wait_all();   // bulk stores must be complete before the CTA exits
   }
@@ -412,11 +527,19 @@ int gemm_tap(const vc_gemm_desc& d, cudaStream_t stream) {
                             (reinterpret_cast<uintptr_t>(d.gn_part) & 7) == 0),
              "gemm_tap: GroupNorm partial sums need an fp16 output with N %% 32 == 0 and N %% gn_sub == 0 (gn_sub 10 or 8)");
   p.gn_part = reinterpret_cast<float2*>(d.gn_part); p.gn_hp = d.gn_sub / 2; p.gn_nchunks = d.N / 32;
-  // vector epilogue accesses need 32-byte aligned rows (true for every activation on the U-Net / VAE path); anything
+  // vector epilogue stores need 32-byte aligned rows (true for every activation on the U-Net / VAE path); anything
   // else (odd pitches, the 4- and 3-channel output convs) takes the predicated scalar path inside the kernel.  The output
   // and the residual are judged separately: the residual is added in registers before any store path runs.
   p.vec_ok = ((reinterpret_cast<uintptr_t>(optr) & 31) == 0) && ((long long)d.ldo * esz) % 32 == 0 ? 1 : 0;
-  p.res_vec = d.res && ((reinterpret_cast<uintptr_t>(d.res) & 31) == 0) && ((long long)d.ldr * 2) % 32 == 0 ? 1 : 0;
+  p.res_tma = d.res && (reinterpret_cast<uintptr_t>(d.res) & 15) == 0 && d.ldr % 8 == 0 ? 1 : 0;
+  if (p.res_tma) {
+    // the residual tile of 128 rows x 32 columns per box, in the output tile's layout (gemm_common.cuh: epi_offset)
+    uint64_t dims[4] = {(uint64_t)d.N, (uint64_t)d.X, (uint64_t)d.Y, (uint64_t)d.Z};
+    uint64_t str[3] = {(uint64_t)d.ldr * 2, (uint64_t)d.ldr * 2 * d.X, (uint64_t)d.ldr * 2 * d.X * d.Y};
+    uint32_t box[4] = {32, (uint32_t)d.bx, (uint32_t)d.by, 1};
+    int rc = encode_tmap_f16(&p.tmap_res, d.res, 4, dims, str, box, 64);
+    if (rc) return rc;
+  }
   {
     // TMA-store epilogue: fp16 output whose width is whole 32-column chunks and whose rows are 16-byte aligned
     const int n_out = d.geglu ? d.N / 2 : d.N;
