@@ -208,6 +208,13 @@ int vc_ddim_update(const float* x, const float* v_cond, const float* v_uncond, c
  * replaces: lvdm/models/samplers/ddim_multiplecond.py:227-236 (+ the shared tail :238-287) */
 int vc_ddim_update3(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img,
                     const float* noise, float* x_prev, float* pred_x0, int64_t n, const vc_ddim_scalars* s, void* ws /* 4 * 1025 doubles */, void* stream);
+/* DPM-Solver++(2M) step (INTEGRATION.md "Samplers"): the DDIM update above (two-way, or three-way when v_uncond_img is not null),
+ * x_ddim, then x_prev = x_ddim + c_hist (x0 - x0_hist) with x0 = sqrt_ac_t x - sqrt_1mac_t v before the dynamic rescale; x0_hist
+ * (n floats, read only when c_hist != 0) is overwritten with this step's x0.  c_hist = 0 gives vc_ddim_update's x_prev bit for bit.
+ * New functionality (the reference has only DDIM). */
+int vc_dpm_update(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img,
+                  const float* noise, float* x0_hist, float* x_prev, float* pred_x0, int64_t n, const vc_ddim_scalars* s, float c_hist,
+                  void* ws /* 4 * 1025 doubles */, void* stream);
 
 /* ---- multi-GPU: frame <-> site layout exchange over NVLink peer memory ------------------------------------------------
  * New functionality (the reference is single-GPU, SURVEY.md 8e).  The frame-sharded U-Net runs its spatial ops on

@@ -351,6 +351,75 @@ int ddim_update(const float* x, const float* v_cond, const float* v_uncond, cons
 }
 
 // ------------------------------------------------------------------------------------------------
+// DPM-Solver++(2M) update (INTEGRATION.md "Samplers"): the DDIM step above, x_ddim, plus the multistep correction
+//   x_prev = x_ddim + c_hist (x0 - x0_hist),   x0 = sqrt_ac_t x - sqrt_1mac_t v  (before the dynamic rescale)
+// x0_hist holds the previous step's x0 and is overwritten with this step's.  c_hist = 0 is a first-order step: x_prev is x_ddim
+// bit for bit and x0_hist is not read (it may be uninitialised on the first step).  x_ddim is ddim_apply_kernel's expression.
+// ------------------------------------------------------------------------------------------------
+__global__ void dpm_apply_kernel(const float* __restrict__ x, const float* __restrict__ vc_, const float* __restrict__ vu,
+                                 const float* __restrict__ vi, float cfg_img,
+                                 const float* __restrict__ noise, float* __restrict__ x0_hist, float* __restrict__ x_prev,
+                                 float* __restrict__ pred_x0, long long n, vc_ddim_scalars s, float c_hist, const double* ws, int stat_blocks) {
+  float factor = 1.f;
+  if (s.use_cfg && s.guidance_rescale > 0.f) {
+    __shared__ double tot[4];
+    if (threadIdx.x < 4) {
+      double a = 0;
+      for (int b = 0; b < stat_blocks; ++b) a += ws[4 + 4 * b + threadIdx.x];
+      tot[threadIdx.x] = a;
+    }
+    __syncthreads();
+    const double dn = (double)n;
+    const double var_t = (tot[1] - tot[0] * tot[0] / dn) / (dn - 1.0);
+    const double var_c = (tot[3] - tot[2] * tot[2] / dn) / (dn - 1.0);
+    factor = (float)sqrt(var_t > 0 ? var_t : 0.0) / (float)sqrt(var_c > 0 ? var_c : 0.0);
+  }
+  const float rescale = s.prev_scale_t / s.scale_t;
+  // eta = 1 from a = 0: 1 - a' - sigma^2 is 0 in exact arithmetic and can round to -2e-8 (4 uniform_trailing steps), where
+  // ddim_apply_kernel's sqrtf gives NaN; clamped here, the same bits wherever it is >= 0
+  const float dir_c = sqrtf(fmaxf(1.f - s.a_prev - s.sigma_t * s.sigma_t, 0.f));
+  const float sq_ap = sqrtf(s.a_prev);
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const float c = vc_[i];
+    float m = c;
+    if (s.use_cfg) {
+      const float u = vu[i];
+      m = cfg_combine(c, u, vi, i, s.cfg_scale, cfg_img);
+      if (s.guidance_rescale > 0.f) m = s.guidance_rescale * (m * factor) + (1.f - s.guidance_rescale) * m;
+    }
+    const float xi = x[i];
+    const float e_t = s.sqrt_ac_t * m + s.sqrt_1mac_t * xi;
+    float p0 = s.sqrt_ac_t * xi - s.sqrt_1mac_t * m;
+    const float x0 = p0;
+    p0 *= rescale;
+    pred_x0[i] = p0;
+    const float x_ddim = sq_ap * p0 + dir_c * e_t + s.sigma_t * noise[i];
+    x_prev[i] = c_hist != 0.f ? __fmaf_rn(c_hist, x0 - x0_hist[i], x_ddim) : x_ddim;
+    x0_hist[i] = x0;
+  }
+}
+int dpm_update(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img, const float* noise,
+               float* x0_hist, float* x_prev, float* pred_x0, long long n, const vc_ddim_scalars& s, float c_hist, double* ws,
+               cudaStream_t stream) {
+  VC_REQUIRE(x && v_cond && noise && x0_hist && x_prev && pred_x0 && ws && n > 1, "dpm_update: bad args");
+  VC_REQUIRE(!s.use_cfg || v_uncond, "dpm_update: CFG needs the unconditional output");
+  VC_REQUIRE(!v_uncond_img || s.use_cfg, "dpm_update: the image-only branch is only defined with CFG on");
+  VC_REQUIRE(x0_hist != x_prev && x0_hist != pred_x0 && x0_hist != x && x_prev != pred_x0, "dpm_update: x0_hist, x_prev and pred_x0 must not alias");
+  VC_REQUIRE(isfinite(c_hist), "dpm_update: c_hist must be finite");
+  // the statistics grid of ddim_update (reproducible mode included), so both updates reduce the same partial sums in the same order
+  int blocks = (int)min(s.reproducible ? (long long)DDIM_REPRO_BLOCKS : (long long)sm_count() * 4, (n + 255) / 256);
+  if (blocks > DDIM_MAX_BLOCKS) blocks = DDIM_MAX_BLOCKS;
+  if (s.use_cfg && s.guidance_rescale > 0.f) {
+    ddim_stats_kernel<<<blocks, 256, 0, stream>>>(v_cond, v_uncond, v_uncond_img, n, s.cfg_scale, cfg_img, ws);
+    VC_CHECK_CUDA(cudaGetLastError());
+  }
+  dpm_apply_kernel<<<blocks, 256, 0, stream>>>(x, v_cond, v_uncond, v_uncond_img, cfg_img, noise, x0_hist, x_prev, pred_x0, n, s, c_hist,
+                                               ws, blocks);
+  VC_CHECK_CUDA(cudaGetLastError());
+  return VC_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
 // row softmax (fp32 scores -> fp16 probabilities) for the VAE's single-head d=512 AttnBlock (ae_modules.py:66-68)
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restrict__ x, long long cols, float scale, __half* __restrict__ out) {

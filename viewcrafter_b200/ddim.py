@@ -265,18 +265,20 @@ class DDIMSampler(object):
         return noise.contiguous()
 
     @staticmethod
-    def _fused_update(x, v_c, v_u, noise, sc, **extra):
+    def _fused_update(x, v_c, v_u, noise, sc, op=None, **extra):
         """One fused update for the batch; the guidance rescale uses per-SAMPLE statistics (utils_diffusion.py:147-158: std over every axis but
-        the batch axis) while the kernel reduces over its whole input, so a batch with guidance rescale is updated sample by sample."""
+        the batch axis) while the kernel reduces over its whole input, so a batch with guidance rescale is updated sample by sample.
+        op: the update (default ops.ddim_update; the DPM-Solver sampler passes ops.dpm_update, whose x0_hist comes in `extra`)."""
+        op = ops.ddim_update if op is None else op
         f = lambda v: None if v is None else v.float().contiguous()
         x, v_c, v_u = f(x), f(v_c), f(v_u)
         extra = {k: (f(v) if isinstance(v, torch.Tensor) else v) for k, v in extra.items()}
         if x.shape[0] == 1 or v_u is None or sc["guidance_rescale"] <= 0.0:
-            return ops.ddim_update(x, v_c, v_u, noise, sc, **extra)
+            return op(x, v_c, v_u, noise, sc, **extra)
         outs = []
         for b in range(x.shape[0]):
             eb = {k: (v[b:b + 1].contiguous() if isinstance(v, torch.Tensor) else v) for k, v in extra.items()}
-            outs.append(ops.ddim_update(x[b:b + 1].contiguous(), v_c[b:b + 1].contiguous(), v_u[b:b + 1].contiguous(), noise[b:b + 1].contiguous(), sc, **eb))
+            outs.append(op(x[b:b + 1].contiguous(), v_c[b:b + 1].contiguous(), v_u[b:b + 1].contiguous(), noise[b:b + 1].contiguous(), sc, **eb))
         return torch.cat([o[0] for o in outs], 0), torch.cat([o[1] for o in outs], 0)
 
     # -- img2img helpers of the reference sampler (ddim.py:288-325) ------------------------------------------------------------

@@ -733,3 +733,30 @@ def ddim_update(x, v_cond, v_uncond, noise, sc: dict, v_uncond_img=None, cfg_img
                                      x_prev.data_ptr(), pred_x0.data_ptr(), x.numel(), C.byref(s), ws.data_ptr(), _stream()),
           "vc_ddim_update")
     return x_prev, pred_x0
+
+
+def dpm_update(x, v_cond, v_uncond, noise, sc: dict, x0_hist, v_uncond_img=None, cfg_img: float = 0.0):
+    """One DPM-Solver++(2M) step (vc_dpm_update): ddim_update's x_{t-1}, plus sc["c_hist"] * (x0 - x0_hist) where x0 is this step's x0
+    prediction before the dynamic rescale.  x0_hist (fp32, x's shape) holds the previous step's x0, is read only when c_hist != 0 and
+    is overwritten in place with this step's.  Returns (x_prev, pred_x0) like ddim_update."""
+    for t in (x, v_cond, noise, x0_hist) + ((v_uncond_img,) if v_uncond_img is not None else ()):
+        assert t.dtype == torch.float32 and t.is_contiguous() and t.is_cuda
+    assert x0_hist.shape == x.shape
+    s = DdimScalars()
+    use_cfg = v_uncond is not None and sc["cfg_scale"] != 1.0
+    s.cfg_scale, s.guidance_rescale = sc["cfg_scale"], sc["guidance_rescale"] if use_cfg else 0.0
+    s.sqrt_ac_t, s.sqrt_1mac_t = sc["sqrt_ac_t"], sc["sqrt_1mac_t"]
+    s.a_prev, s.sigma_t, s.scale_t, s.prev_scale_t = sc["a_prev"], sc["sigma_t"], sc["scale_t"], sc["prev_scale_t"]
+    s.use_cfg = int(use_cfg)
+    s.reproducible = int(REPRODUCIBLE)
+    key = (x.device, torch.cuda.current_stream().cuda_stream)
+    ws = _ddim_ws.get(key)
+    if ws is None:
+        ws = torch.zeros(4 * 1025, device=x.device, dtype=torch.float64)
+        _ddim_ws[key] = ws
+    x_prev, pred_x0 = torch.empty_like(x), torch.empty_like(x)
+    vi = v_uncond_img if use_cfg else None
+    check(_lib.load().vc_dpm_update(x.data_ptr(), v_cond.data_ptr(), _ptr(v_uncond) if use_cfg else None, _ptr(vi), float(cfg_img),
+                                    noise.data_ptr(), x0_hist.data_ptr(), x_prev.data_ptr(), pred_x0.data_ptr(), x.numel(), C.byref(s),
+                                    float(sc["c_hist"]), ws.data_ptr(), _stream()), "vc_dpm_update")
+    return x_prev, pred_x0

@@ -55,6 +55,25 @@ def ddim_parameters(alphacums: torch.Tensor, ts: np.ndarray, eta: float):
     return sigmas, alphas, alphas_prev
 
 
+def dpm_coefficients(alphacums, ts: np.ndarray, eta: float) -> np.ndarray:
+    """float64 [S]: c of the DPM-Solver++(2M) step of DDIM index j (INTEGRATION.md "Samplers"), which goes from a = alphacums[ts[j]] to
+    a' = alphacums[ts[j - 1]] (alphacums[0] for j = 0) with h_j = lambda(a') - lambda(a), lambda = log(a / (1 - a)) / 2:
+        c_j = sqrt(a') (1 - exp(-(1 + eta) h_j)) / (2 r),   r = h_{j+1} / h_j   (step j + 1 is the one sampled before step j).
+    c_j = 0 -- a first-order (DDIM) step -- on the first step (j = S - 1), the last (j = 0), after a step that started at a = 0
+    (h_{j+1} infinite) and where h_j or h_{j+1} is 0 (repeated timesteps of the "quad" spacing)."""
+    ac = np.asarray(alphacums, dtype=np.float64)
+    a = ac[ts]
+    a_prev = np.concatenate([ac[0:1], a[:-1]])
+    with np.errstate(divide="ignore"):
+        lam = lambda v: 0.5 * (np.log(v) - np.log1p(-v))
+        h = lam(a_prev) - lam(a)
+    c = np.zeros(len(ts), dtype=np.float64)
+    for j in range(1, len(ts) - 1):
+        if np.isfinite(h[j + 1]) and h[j + 1] != 0 and h[j] != 0:
+            c[j] = np.sqrt(a_prev[j]) * -np.expm1(-(1.0 + eta) * h[j]) * h[j] / (2.0 * h[j + 1])
+    return c
+
+
 def f32(v) -> float:
     """The value torch.full(size, v) would hold (float32 rounding of a python/numpy/tensor scalar)."""
     return float(np.float32(float(v)))

@@ -26,6 +26,10 @@ import torch
 from . import ops, parallel
 from .ddim import DDIMSampler, check_row_replay
 from .ddim_multiplecond import DDIMSampler as DDIMSampler_multicond
+from .dpm_solver import DPMSolverSampler, DPMSolverSamplerMultiCond, check_eta
+
+# image_guided_synthesis(sampler=...) -> (two-way sampler class, three-way sampler class)
+SAMPLERS = {"ddim": (DDIMSampler, DDIMSampler_multicond), "dpmpp_2m": (DPMSolverSampler, DPMSolverSamplerMultiCond)}
 
 
 def _vae_sharded(model) -> bool:
@@ -48,28 +52,36 @@ def get_latent_z(model, videos):
 def image_guided_synthesis(model, prompts, videos, noise_shape, n_samples=1, ddim_steps=50, ddim_eta=1.,
                            unconditional_guidance_scale=1.0, cfg_img=None, fs=None, text_input=False, multiple_cond_cfg=False,
                            timestep_spacing='uniform', guidance_rescale=0.0, condition_index=None, batch_cfg=True, cuda_graph=True,
-                           reproducible=None, **kwargs):
+                           reproducible=None, sampler="ddim", **kwargs):
     """reproducible: True / False switches viewcrafter_b200's reproducible mode (ops.set_reproducible) for this call and restores the
-    previous setting afterwards; None leaves the process setting as it is."""
+    previous setting afterwards; None leaves the process setting as it is.
+    sampler: "ddim" (the reference's DDIMSampler) or "dpmpp_2m" (dpm_solver.DPMSolverSampler / DPMSolverSamplerMultiCond, which takes
+    ddim_eta 0 or 1 only; INTEGRATION.md "Samplers")."""
+    if sampler not in SAMPLERS:
+        raise ValueError(f"unknown sampler {sampler!r}; choose one of {sorted(SAMPLERS)}")
+    if sampler == "dpmpp_2m":
+        check_eta(ddim_eta)                               # before the conditioning is computed
     if reproducible is None:
         return _synthesis(model, prompts, videos, noise_shape, n_samples, ddim_steps, ddim_eta, unconditional_guidance_scale, cfg_img, fs,
-                          text_input, multiple_cond_cfg, timestep_spacing, guidance_rescale, condition_index, batch_cfg, cuda_graph, **kwargs)
+                          text_input, multiple_cond_cfg, timestep_spacing, guidance_rescale, condition_index, batch_cfg, cuda_graph,
+                          sampler=sampler, **kwargs)
     prev = ops.set_reproducible(reproducible)
     try:
         return _synthesis(model, prompts, videos, noise_shape, n_samples, ddim_steps, ddim_eta, unconditional_guidance_scale, cfg_img, fs,
-                          text_input, multiple_cond_cfg, timestep_spacing, guidance_rescale, condition_index, batch_cfg, cuda_graph, **kwargs)
+                          text_input, multiple_cond_cfg, timestep_spacing, guidance_rescale, condition_index, batch_cfg, cuda_graph,
+                          sampler=sampler, **kwargs)
     finally:
         ops.set_reproducible(prev)
 
 
 def _synthesis(model, prompts, videos, noise_shape, n_samples, ddim_steps, ddim_eta, unconditional_guidance_scale, cfg_img, fs, text_input,
-               multiple_cond_cfg, timestep_spacing, guidance_rescale, condition_index, batch_cfg, cuda_graph, **kwargs):
+               multiple_cond_cfg, timestep_spacing, guidance_rescale, condition_index, batch_cfg, cuda_graph, sampler="ddim", **kwargs):
     if getattr(model, "_replicas", None) is not None:
         check_row_replay(kwargs)                          # before any collective, on every rank alike
     unet = getattr(getattr(model, "model", None), "diffusion_model", None)
     if cuda_graph and hasattr(unet, "enable_cuda_graph") and next(unet.parameters()).is_cuda:
         unet.enable_cuda_graph()              # the ~100 forwards of a clip share shapes, weights and context: capture once, replay
-    ddim_sampler = DDIMSampler(model, batch_cfg=batch_cfg) if not multiple_cond_cfg else DDIMSampler_multicond(model, batch_cfg=batch_cfg)
+    ddim_sampler = SAMPLERS[sampler][bool(multiple_cond_cfg)](model, batch_cfg=batch_cfg)
     batch_size = noise_shape[0]
     fs = torch.tensor([fs] * batch_size, dtype=torch.long, device=model.device)
 
