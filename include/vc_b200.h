@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define VC_B200_ABI_VERSION 8
+#define VC_B200_ABI_VERSION 9
 
 int vc_abi_version(void);
 const char* vc_last_error(void);
@@ -56,8 +56,9 @@ typedef struct vc_gemm_desc {
    * out[r,n] = rstd[r] * (acc[r,n] - mean[r] * ln_colsum[n]) + bias[n].  NULL = plain GEMM.  num_taps must be 1. */
   const float* ln_stats;             /* [rows][2] fp32 (mean, rstd) from vc_layernorm_stats                */
   const float* ln_colsum;            /* [N] fp32: sum_k w[n,k] of the fp16 weights                         */
-  /* optional by-product for the NEXT LayerNorm: partial (sum, sumsq) of the fp16-rounded output, per row and 32-column chunk,
-   * ln_part[(n/32) * M + row][2]; plain fp16 [M,N] outputs with N % 32 == 0 only.  vc_layernorm_stats_from_parts finishes them. */
+  /* optional by-product for the NEXT LayerNorm: per row and 32-column chunk of the fp16-rounded output, its sum and M2 (the sum of
+   * squared deviations about the chunk's own mean, sum / 32), ln_part[(n/32) * M + row][2]; plain fp16 [M,N] outputs with N % 32 == 0
+   * only.  vc_layernorm_stats_from_parts finishes them.  (ABI 8 and older held (sum, sum of squares).) */
   float* ln_part;
   /* optional output pitches in elements along Y and Z (0 = dense: ldo*X and ldo*X*Y); non-dense outputs require an fp16 output
    * with N % 32 == 0 and no residual.  Upsample (F.interpolate nearest x2, openaimodel3d.py:80-106) + 3x3 conv runs as four
@@ -162,7 +163,8 @@ int vc_groupnorm_apply_leaves(const void* x1, int32_t C1, const void* x2, int32_
 /* statistics half of nn.LayerNorm: stats[row] = (mean, 1/sqrt(var + eps)) in fp32; the normalisation is applied by the
  * consuming vc_gemm_tap (ln_stats / ln_colsum), so the normalised activation is never written to memory */
 int vc_layernorm_stats(const void* x, int64_t rows, int32_t C, float eps, float* stats, void* stream);
-/* the same statistics from the partial sums a producing vc_gemm_tap left in ln_part ([C/32][rows][2] fp32): no re-read of x */
+/* the same statistics from the (sum, M2) records a producing vc_gemm_tap left in ln_part ([C/32][rows][2] fp32), merged in chunk
+ * order by Chan's formula: no re-read of x */
 int vc_layernorm_stats_from_parts(const float* parts, int64_t rows, int32_t C, float eps, float* stats, void* stream);
 /* nn.LayerNorm over the last dim (attention.py:233-235), fp16 in/out, fp32 statistics */
 int vc_layernorm(const void* x, int64_t rows, int32_t C, const float* gamma, const float* beta, float eps, void* out,

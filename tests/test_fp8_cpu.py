@@ -67,11 +67,18 @@ def test_pack_fp8_upconv_presummed_taps():
         assert _same(q, q_ref) and torch.equal(s, s_ref)
 
 
-def test_gemm_desc_abi():
+def test_gemm_desc_abi_version_9():
+    """ABI 9: the descriptor's FP8 fields, and the version both the binding and include/vc_b200.h declare (9 since ln_part records hold
+    (sum, M2 about the chunk mean))."""
+    import os
+    import re
     from viewcrafter_b200 import _lib
     names = [f[0] for f in _lib.GemmDesc._fields_]
     assert names[-4:] == ["peer", "fp8", "w_scale", "a_amax"]
-    assert _lib.ABI_VERSION == 8
+    assert _lib.ABI_VERSION == 9
+    header = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "include", "vc_b200.h")
+    with open(header) as f:
+        assert int(re.search(r"#define VC_B200_ABI_VERSION (\d+)", f.read()).group(1)) == _lib.ABI_VERSION
     d = _lib.GemmDesc()
     assert d.fp8 == 0 and not d.w_scale and not d.a_amax
     assert "vc_absmax_f16" in _lib.SIGNATURES

@@ -94,7 +94,7 @@ struct GemmParams {
   int geglu;
   const float* ln_stats;   // folded LayerNorm: per-row (mean, rstd); nullptr = plain
   const float* ln_colsum;  // folded LayerNorm: per-column sum of the (gamma-scaled) weights
-  float2* ln_part;         // optional: per (32-column chunk, row) partial (sum, sumsq) of the fp16-rounded outputs, [N/32][ln_rows]:
+  float2* ln_part;         // optional: per (32-column chunk, row) (sum, M2 about the chunk mean) of the fp16-rounded outputs, [N/32][ln_rows]:
   long long ln_rows;       //   the LayerNorm statistics of the tensor this GEMM writes, gathered while it is still in registers
   float2* gn_part;         // optional: GroupNorm partial (sum, sumsq) of the fp16-rounded outputs per (32-row block, 32-column chunk, piece):
   int gn_hp;               //   [m_tile * 4 + quadrant][N / 32][4]; a chunk is cut at the boundaries of gn_sub = 2 * gn_hp channel sub-groups
@@ -315,11 +315,16 @@ __device__ __forceinline__ void epi_stats_row32(const GemmParams& p, const EpiTi
     f[2 * e] = r.x; f[2 * e + 1] = r.y;
   }
   if (p.ln_part) {                                 // LayerNorm statistics of the OUTPUT row, as stored (fp16-rounded)
-    float s = 0.f, q = 0.f;
+    // (sum, M2): M2 is taken about the chunk's own mean, so it does not cancel when the row's |mean| >> std
+    float s = 0.f;
+#pragma unroll
+    for (int e = 0; e < 32; e += 2) s += f[e] + f[e + 1];
+    const float m = s * (1.f / 32.f);
+    float q = 0.f;
 #pragma unroll
     for (int e = 0; e < 32; e += 2) {
-      s += f[e] + f[e + 1];
-      q = fmaf(f[e], f[e], fmaf(f[e + 1], f[e + 1], q));
+      const float a = f[e] - m, b = f[e + 1] - m;
+      q = fmaf(a, a, fmaf(b, b, q));
     }
     if (t.row_ok) p.ln_part[(long long)(nb >> 5) * p.ln_rows + t.orow] = make_float2(s, q);
   }

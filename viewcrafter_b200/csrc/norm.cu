@@ -286,12 +286,14 @@ int groupnorm_nhwc(const __half* x1, int C1, const __half* x2, int C2, int sampl
 }
 
 // Split form for statistics that span several GPUs (site-sharded 5-D GroupNorm): pass 1 leaves (sum, sumsq) per group in
-// stats[samples][32][2]; the caller all-reduces that tiny buffer; pass 2 normalises with the global row count.
+// stats[samples][32][2]; the caller all-reduces that tiny buffer; pass 2 normalises with the global row count.  The per-CTA
+// records are summed in fp64 and rounded once, as the single-GPU apply pass sums them: an fp32 running sum over ~260 records
+// lost enough of the sum of squares to break the output bound at |mean| = 64 std.
 __global__ void gn_finalize_kernel(const float* __restrict__ partial, int splits, float* __restrict__ stats) {
   const int sample = blockIdx.x, t = threadIdx.x;   // 64 threads
-  float acc = 0.f;
+  double acc = 0.0;
   for (int sp = 0; sp < splits; ++sp) acc += partial[((long long)sample * splits + sp) * 64 + t];
-  stats[sample * 64 + t] = acc;
+  stats[sample * 64 + t] = (float)acc;
 }
 
 int groupnorm_stats(const __half* x1, int C1, const __half* x2, int C2, int samples, long long rows_per_sample, float* stats,
@@ -750,25 +752,34 @@ __global__ void __launch_bounds__(256) ln_stats_unrolled_kernel(const __half* __
   }
 }
 
-// (mean, rstd) per row from the per-32-column partial sums a producing GEMM left in parts[C/32][rows] (vc_gemm_desc::ln_part):
-// reads C/32 * 8 bytes per row instead of 2 C bytes -- the LayerNorm statistics pass without re-reading the activation.
-__global__ void __launch_bounds__(256) ln_finalize_kernel(const float2* __restrict__ parts, long long rows, int nchunks, float invC, float eps,
+// (mean, rstd) per row from the per-32-column records a producing GEMM left in parts[C/32][rows] (vc_gemm_desc::ln_part): reads
+// C/32 * 8 bytes per row instead of 2 C bytes -- the LayerNorm statistics pass without re-reading the activation.  A record is
+// (sum, M2 about the chunk's mean); the chunks are merged in index order with Chan's formula,
+//   mean = sum_c s_c / C,   M2 = sum_c M2_c + 32 sum_c (s_c / 32 - mean)^2,
+// so no term cancels when |mean| >> std.  The mean is a true division: a constant row gets its value back, and variance 0.
+__global__ void __launch_bounds__(256) ln_finalize_kernel(const float2* __restrict__ parts, long long rows, int nchunks, float eps,
                                                           float2* __restrict__ stats) {
   const long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (row >= rows) return;
-  float s = 0.f, q = 0.f;
+  const float2* p = parts + row;
+  float s = 0.f;
+  for (int c = 0; c < nchunks; ++c) s += __ldg(p + (long long)c * rows).x;
+  const float C = 32.f * (float)nchunks;
+  const float mean = s / C;
+  float m2 = 0.f, between = 0.f;
   for (int c = 0; c < nchunks; ++c) {
-    const float2 v = __ldg(parts + (long long)c * rows + row);
-    s += v.x; q += v.y;
+    const float2 v = __ldg(p + (long long)c * rows);
+    const float d = v.x * (1.f / 32.f) - mean;
+    m2 += v.y;
+    between = fmaf(d, d, between);
   }
-  const float mean = s * invC;
-  const float var = fmaxf(q * invC - mean * mean, 0.f);
+  const float var = fmaf(32.f, between, m2) / C;
   stats[row] = make_float2(mean, rsqrtf(var + eps));
 }
 
 int layernorm_stats_from_parts(const float* parts, long long rows, int C, float eps, float* stats, cudaStream_t stream) {
   VC_REQUIRE(parts && stats && rows > 0 && C % 32 == 0, "layernorm_stats_from_parts: bad args");
-  ln_finalize_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const float2*>(parts), rows, C / 32, 1.f / (float)C, eps,
+  ln_finalize_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const float2*>(parts), rows, C / 32, eps,
                                                                         reinterpret_cast<float2*>(stats));
   VC_CHECK_CUDA(cudaGetLastError());
   return VC_OK;
