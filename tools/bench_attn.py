@@ -11,7 +11,6 @@ def t(fn, reps=5):
     e1.record(); torch.cuda.synchronize()
     return e0.elapsed_time(e1) / reps * 1e-3
 T = 25
-print("VC_ATTN_EXP =", os.environ.get("VC_ATTN_EXP", "f16x2"))
 for name, HW, heads in (("l0", 9216, 5), ("l1", 2304, 10), ("l2", 576, 20), ("l3", 144, 20)):
     C = heads * 64
     qkv = (torch.randn(T * HW, 3 * C, device="cuda") * 0.7).half()
