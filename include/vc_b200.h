@@ -112,7 +112,7 @@ typedef struct vc_attn_desc {
 } vc_attn_desc;
 int vc_flash_attn_d64(const vc_attn_desc* d, void* stream);
 
-/* temporal self-attention over T <= 32 frames per spatial site (TemporalTransformer, attention.py:365-412;
+/* temporal self-attention over 1 <= T <= 128 frames per spatial site (TemporalTransformer, attention.py:365-412;
  * always the naive path in the reference, attention.py:66).  q/k/v rows at (t*sites + site), pitch ld. */
 int vc_temporal_attn(const void* q, const void* k, const void* v, int32_t ld, void* out, int32_t ldo, int32_t T,
                      int64_t sites, int32_t heads, float scale, void* stream);

@@ -47,7 +47,8 @@ int layernorm_stats_from_parts(const float* parts, long long rows, int C, float 
 int layernorm_rows(const __half* x, long long rows, int C, const float* gamma, const float* beta, float eps, __half* out,
                    cudaStream_t stream);
 
-// Temporal self-attention over T<=32 frames per spatial site; qkv rows are [T*sites, ld] with q|k|v at column offsets.
+// Temporal self-attention over 1 <= T <= 128 frames per spatial site (T <= 32 and 33..128 run different kernels); qkv rows are
+// [T*sites, ld] with q|k|v at column offsets.
 int temporal_attn(const __half* q, const __half* k, const __half* v, int ld, __half* out, int ldo, int T, long long sites,
                   int heads, float scale, cudaStream_t stream);
 

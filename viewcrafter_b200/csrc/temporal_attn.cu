@@ -1,8 +1,8 @@
-// Temporal self-attention over T <= 32 frames per spatial site (TemporalTransformer attn1/attn2,
+// Temporal self-attention over T <= 128 frames per spatial site (TemporalTransformer attn1/attn2,
 // lvdm/modules/attention.py:81-126 with N = T, batch = H*W sites; the reference always takes the naive
 // einsum-softmax-einsum path here, attention.py:66).
 //
-// The problem per (site, head) is a 25x25x64 attention: far below the 64-row granularity of a wgmma and
+// T <= 32: the problem per (site, head) is a 25x25x64 attention: far below the 64-row granularity of a wgmma and
 // HBM-bound (3 x T x 128 B in, T x 128 B out per pair), so it runs on warp-level mma.sync m16n8k16 tiles: one warp
 // per (site, head), Q/K/V staged in shared memory with 16-byte coalesced loads, S and O accumulators in registers,
 // softmax on the accumulator fragments, P re-used in registers as the A operand of P.V (no smem round trip).
@@ -181,11 +181,219 @@ __global__ void __launch_bounds__(TA_WARPS * 32) temporal_attn_kernel(const __ha
   }
 }
 
+// ------------------------------------------------------------------------------------------------ 33 <= T <= 128
+// Long clips.  One CTA of TL_WARPS warps runs one (site, head) pair at a time: Q, K and V (KT*16 rows, zero-filled past T) sit in
+// shared memory, warp w computes the query tiles w, w + TL_WARPS, ... of 16 rows with the whole score row (KT*16 keys, at most 64 fp32
+// per thread) in registers, so the softmax is the single max / exp / sum pass of the T <= 32 kernel and the arithmetic per element is
+// the same.  The pair is HBM-bound (T/2 FLOP per byte), so the CTA keeps the next pair's Q/K/V in flight with cp.async while it
+// computes the current one (TL_STAGES buffers, grid-stride over the pairs).
+static constexpr int TL_WARPS = 4;
+static constexpr int TL_STAGES = 2;
+static constexpr int TL_MAX_T = 128;
+
+template <int KT>
+struct TlShape {
+  static constexpr int ROWS = KT * 16;                                // padded frames per pair
+  static constexpr int STAGE = 3 * ROWS * TA_PITCH;                   // halves: Q | K | V
+  static constexpr int SMEM = TL_STAGES * STAGE * 2;                  // bytes
+};
+
+__device__ __forceinline__ void cp_async16(void* dst, const void* src, bool valid) {
+  // src-size 0 zero-fills the 16 bytes without reading src: frames >= T become zero rows
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst)), "l"(src), "r"(valid ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+template <int KT>
+__device__ __forceinline__ void tl_load_pair(__half* stage, const __half* __restrict__ q, const __half* __restrict__ k,
+                                             const __half* __restrict__ v, int ld, int T, long long sites, int heads, long long pair) {
+  constexpr int ROWS = TlShape<KT>::ROWS;
+  const long long site = pair / heads;
+  const int head = (int)(pair % heads);
+  static_assert(TL_WARPS * 32 == 16 * 8, "one pass copies 16 rows of 8 chunks");
+#pragma unroll
+  for (int j = 0; j < 3 * KT; ++j) {                                 // pass j: rows 16 (j % KT) .. + 15 of tensor j / KT
+    const int which = j / KT, r = 16 * (j % KT) + (threadIdx.x >> 3), c = (threadIdx.x & 7) * 8;
+    const __half* src = which == 0 ? q : which == 1 ? k : v;
+    const bool valid = r < T;
+    const long long off = valid ? ((long long)r * sites + site) * ld + head * 64 + c : 0;
+    cp_async16(stage + (which * ROWS + r) * TA_PITCH + c, src + off, valid);
+  }
+}
+
+template <int KT>
+__global__ void __launch_bounds__(TL_WARPS * 32, 2) temporal_attn_long_kernel(const __half* __restrict__ q, const __half* __restrict__ k,
+                                                                           const __half* __restrict__ v, int ld, __half* __restrict__ out,
+                                                                           int ldo, int T, long long sites, int heads, float scale_log2) {
+  constexpr int ROWS = TlShape<KT>::ROWS, STAGE = TlShape<KT>::STAGE;
+  extern __shared__ __align__(16) __half tl_smem[];
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int g = lane >> 2, tg = lane & 3;
+  const int mat = lane >> 3, mr = lane & 7;
+  const int lrow = lane >> 3, lchunk = (lane & 7) * 8;
+  const long long pairs = sites * heads;
+
+  // prologue: the first TL_STAGES - 1 pairs of this CTA
+#pragma unroll
+  for (int s = 0; s < TL_STAGES - 1; ++s) {
+    const long long pair = blockIdx.x + (long long)s * gridDim.x;
+    if (pair < pairs) tl_load_pair<KT>(tl_smem + s * STAGE, q, k, v, ld, T, sites, heads, pair);
+    cp_async_commit();
+  }
+  int stage = 0;
+  for (long long pair = blockIdx.x; pair < pairs; pair += gridDim.x) {
+    {
+      const long long ahead = pair + (long long)(TL_STAGES - 1) * gridDim.x;
+      if (ahead < pairs) tl_load_pair<KT>(tl_smem + ((stage + TL_STAGES - 1) % TL_STAGES) * STAGE, q, k, v, ld, T, sites, heads, ahead);
+      cp_async_commit();
+    }
+    cp_async_wait<TL_STAGES - 1>();
+    __syncthreads();
+    __half* Qs = tl_smem + stage * STAGE;
+    const __half* Ks = Qs + ROWS * TA_PITCH;
+    const __half* Vs = Ks + ROWS * TA_PITCH;
+    const long long site = pair / heads;
+    const int head = (int)(pair % heads);
+
+    for (int mt = w; mt < KT; mt += TL_WARPS) {
+      // ---- S = Q K^T : [16 x ROWS], k = 64 ----
+      float s[2 * KT][4];
+#pragma unroll
+      for (int ni = 0; ni < 2 * KT; ++ni)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) s[ni][e] = 0.f;
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        uint32_t a[4];
+        ldsm_x4(a[0], a[1], a[2], a[3], Qs + (mt * 16 + (mat & 1) * 8 + mr) * TA_PITCH + kk * 16 + (mat >> 1) * 8);
+#pragma unroll
+        for (int np = 0; np < KT; ++np) {                      // two n-tiles (16 keys) per ldmatrix.x4
+          uint32_t b0, b1, b2, b3;
+          ldsm_x4(b0, b1, b2, b3, Ks + (np * 16 + (mat >> 1) * 8 + mr) * TA_PITCH + kk * 16 + (mat & 1) * 8);
+          mma16816(s[2 * np], a, b0, b1);
+          mma16816(s[2 * np + 1], a, b2, b3);
+        }
+      }
+
+      // ---- softmax over the key axis; each thread owns rows g / g + 8 of the tile ----
+      uint32_t p[KT][4];                                       // P as A fragments per k-step of 16 keys
+      float inv_l[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {                            // h = 0: row g, h = 1: row g + 8
+        float mx = -INFINITY;
+#pragma unroll
+        for (int ni = 0; ni < 2 * KT; ++ni)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = ni * 8 + 2 * tg + e;
+            float val = s[ni][2 * h + e];
+            if (col >= T) val = -INFINITY;
+            s[ni][2 * h + e] = val;
+            mx = fmaxf(mx, val);
+          }
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+        const float off = mx * scale_log2;
+        float l = 0.f;
+#pragma unroll
+        for (int ni = 0; ni < 2 * KT; ++ni)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const float pv = exp2f(fmaf(s[ni][2 * h + e], scale_log2, -off));
+            s[ni][2 * h + e] = pv;
+            l += pv;
+          }
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        inv_l[h] = 1.f / l;
+      }
+#pragma unroll
+      for (int kk = 0; kk < KT; ++kk) {
+        p[kk][0] = pack_half2(s[2 * kk][0], s[2 * kk][1]);
+        p[kk][1] = pack_half2(s[2 * kk][2], s[2 * kk][3]);
+        p[kk][2] = pack_half2(s[2 * kk + 1][0], s[2 * kk + 1][1]);
+        p[kk][3] = pack_half2(s[2 * kk + 1][2], s[2 * kk + 1][3]);
+      }
+
+      // ---- O = P V : [16 x 64], k = ROWS keys (V rows >= T are zero and their P is 0) ----
+      float o[8][4];
+#pragma unroll
+      for (int ni = 0; ni < 8; ++ni)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) o[ni][e] = 0.f;
+#pragma unroll
+      for (int kk = 0; kk < KT; ++kk) {
+#pragma unroll
+        for (int np = 0; np < 4; ++np) {                       // two d-tiles (16 columns) per ldmatrix.x4.trans
+          uint32_t b0, b1, b2, b3;
+          ldsm_x4_t(b0, b1, b2, b3, Vs + (kk * 16 + (mat & 1) * 8 + mr) * TA_PITCH + np * 16 + (mat >> 1) * 8);
+          mma16816(o[2 * np], p[kk], b0, b1);
+          mma16816(o[2 * np + 1], p[kk], b2, b3);
+        }
+      }
+
+      // ---- O / l -> this warp's own Q rows -> coalesced 16-byte row stores ----
+      __syncwarp();
+      __half* Os = Qs + mt * 16 * TA_PITCH;
+#pragma unroll
+      for (int ni = 0; ni < 8; ++ni) {
+        *reinterpret_cast<uint32_t*>(Os + g * TA_PITCH + ni * 8 + 2 * tg) = pack_half2(o[ni][0] * inv_l[0], o[ni][1] * inv_l[0]);
+        *reinterpret_cast<uint32_t*>(Os + (g + 8) * TA_PITCH + ni * 8 + 2 * tg) = pack_half2(o[ni][2] * inv_l[1], o[ni][3] * inv_l[1]);
+      }
+      __syncwarp();
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int r = lrow + 4 * i, t = mt * 16 + r;
+        if (t < T)
+          *reinterpret_cast<uint4*>(out + ((long long)t * sites + site) * ldo + head * 64 + lchunk) =
+              *reinterpret_cast<const uint4*>(Os + r * TA_PITCH + lchunk);
+      }
+    }
+    __syncthreads();                                           // this stage is refilled by the next iteration's prefetch
+    stage = (stage + 1) % TL_STAGES;
+  }
+  cp_async_wait<0>();
+}
+
+template <int KT>
+static int temporal_attn_long(const __half* q, const __half* k, const __half* v, int ld, __half* out, int ldo, int T, long long sites,
+                              int heads, float scale_log2, cudaStream_t stream) {
+  constexpr int SMEM = TlShape<KT>::SMEM;
+  static DeviceOnce configured;
+  if (device_once_needed(configured)) {
+    VC_CHECK_CUDA(cudaFuncSetAttribute(temporal_attn_long_kernel<KT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    device_once_mark(configured);
+  }
+  int per_sm = 0;
+  VC_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, temporal_attn_long_kernel<KT>, TL_WARPS * 32, SMEM));
+  VC_REQUIRE(per_sm >= 1, "temporal_attn: the T=%d kernel does not fit on an SM", T);
+  const long long pairs = sites * heads;
+  VC_REQUIRE(pairs >= 1, "temporal_attn: sites=%lld heads=%d", sites, heads);
+  long long blocks = (long long)per_sm * sm_count();                // grid-stride beyond one resident wave
+  if (blocks > pairs) blocks = pairs;
+  temporal_attn_long_kernel<KT><<<(unsigned)blocks, TL_WARPS * 32, SMEM, stream>>>(q, k, v, ld, out, ldo, T, sites, heads, scale_log2);
+  VC_CHECK_CUDA(cudaGetLastError());
+  return VC_OK;
+}
+
 int temporal_attn(const __half* q, const __half* k, const __half* v, int ld, __half* out, int ldo, int T, long long sites,
                   int heads, float scale, cudaStream_t stream) {
+  VC_REQUIRE(T >= 1 && T <= TL_MAX_T, "temporal_attn: T=%d unsupported (1..%d)", T, TL_MAX_T);
   VC_REQUIRE(q && k && v && out, "temporal_attn: null pointer");
-  VC_REQUIRE(T >= 1 && T <= 32, "temporal_attn: T=%d unsupported (1..32)", T);
   VC_REQUIRE(ld % 8 == 0 && ldo % 8 == 0, "temporal_attn: pitches must be multiples of 8");
+  if (T > 32) {
+    const float sl2 = scale * 1.4426950408889634f;
+    switch ((T + 15) / 16) {
+      case 3: return temporal_attn_long<3>(q, k, v, ld, out, ldo, T, sites, heads, sl2, stream);
+      case 4: return temporal_attn_long<4>(q, k, v, ld, out, ldo, T, sites, heads, sl2, stream);
+      case 5: return temporal_attn_long<5>(q, k, v, ld, out, ldo, T, sites, heads, sl2, stream);
+      case 6: return temporal_attn_long<6>(q, k, v, ld, out, ldo, T, sites, heads, sl2, stream);
+      case 7: return temporal_attn_long<7>(q, k, v, ld, out, ldo, T, sites, heads, sl2, stream);
+      default: return temporal_attn_long<8>(q, k, v, ld, out, ldo, T, sites, heads, sl2, stream);
+    }
+  }
   static DeviceOnce configured;
   if (device_once_needed(configured)) {
     VC_CHECK_CUDA(cudaFuncSetAttribute(temporal_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TA_SMEM));

@@ -10,7 +10,7 @@ libvc_b200.so on channels-last fp16 activations (``rows = (b t) h w``, columns =
     SpatialTransformer  -> GroupNorm, proj_in GEMM, LN, fused-QKV GEMM, wgmma flash attention, out-proj GEMM
                            (+res), LN, q GEMM, text + image cross attention (accumulate), LN, GEGLU GEMM, FF GEMM,
                            proj_out GEMM (+x_in)                                                  (attention.py:249-310)
-    TemporalTransformer -> same with the temporal (T<=32) attention kernel, no transposes: tokens stay in
+    TemporalTransformer -> same with the temporal (T<=128) attention kernels, no transposes: tokens stay in
                            (t, h, w) row order and the kernel strides over t                      (attention.py:313-412)
 """
 from __future__ import annotations
