@@ -618,8 +618,23 @@ def softmax_rows(x: torch.Tensor, scale: float) -> torch.Tensor:
     return out
 
 
+def _rows_view(x: torch.Tensor, rows: int, cols: int, who: str):
+    """The kernels index a row matrix as base + row * stride(0) + column: reject views they would read or write past."""
+    if x.dim() != 2 or x.shape[0] != rows or x.shape[1] < cols or x.stride(1) != 1 or x.stride(0) < x.shape[1]:
+        raise VcError(f"{who}: expected a [{rows}, >= {cols}] row matrix with unit column stride, got shape {tuple(x.shape)} "
+                      f"strides {x.stride()}")
+
+
+def _dense16(x: torch.Tensor, rows: int, who: str):
+    """fp16 [rows, C] rows packed densely (pitch C), 16-byte aligned, C a multiple of 8: the layout the uint4 kernels read."""
+    _chk16(x, who)
+    if x.dim() != 2 or x.shape[0] != rows or not x.is_contiguous() or x.shape[1] % 8 or x.data_ptr() % 16:
+        raise VcError(f"{who}: expected a contiguous, 16-byte aligned fp16 [{rows}, C % 8 == 0] tensor, got shape {tuple(x.shape)} "
+                      f"strides {x.stride()}")
+
+
 def upsample2x(x: torch.Tensor, N: int, H: int, W: int) -> torch.Tensor:
-    _chk16(x, "upsample.x")
+    _dense16(x, N * H * W, "upsample.x")
     Cc = x.shape[1]
     out = torch.empty((N * 4 * H * W, Cc), device=x.device, dtype=torch.float16)
     check(_lib.load().vc_upsample2x_nhwc(x.data_ptr(), out.data_ptr(), N, H, W, Cc, _stream()), "vc_upsample2x_nhwc")
@@ -629,7 +644,7 @@ def upsample2x(x: torch.Tensor, N: int, H: int, W: int) -> torch.Tensor:
 def im2col_s2(x: torch.Tensor, N: int, H: int, W: int, pad_lo: int = 1, pad_hi: Optional[int] = None) -> tuple:
     """stride-2 3x3 patches, zero padding pad_lo (top/left) and pad_hi (bottom/right; default = pad_lo).  U-Net Downsample:
     (1, 1); VAE Downsample: (0, 1) (ae_modules.py:102-106)."""
-    _chk16(x, "im2col.x")
+    _dense16(x, N * H * W, "im2col.x")
     Cc = x.shape[1]
     pad_hi = pad_lo if pad_hi is None else pad_hi
     Ho, Wo = (H + pad_lo + pad_hi - 3) // 2 + 1, (W + pad_lo + pad_hi - 3) // 2 + 1
@@ -639,15 +654,23 @@ def im2col_s2(x: torch.Tensor, N: int, H: int, W: int, pad_lo: int = 1, pad_hi: 
 
 
 def ncthw_to_rows(x: torch.Tensor, out: torch.Tensor, c_off: int = 0):
-    """fp32 [B,C,T,H,W] -> fp16 rows [(B T H W), ld] at channel offset c_off ('b c t h w -> (b t) h w c')."""
+    """fp32 [B,C,T,H,W] -> fp16 rows [(B T H W), ld] at channel offset c_off ('b c t h w -> (b t) h w c').  Only the columns
+    c_off .. c_off + C - 1 of out are written."""
     B, Cc, T, H, W = x.shape
     assert x.dtype == torch.float32 and x.is_contiguous()
+    _chk16(out, "ncthw_to_rows.out")
+    if c_off < 0:
+        raise VcError(f"ncthw_to_rows: c_off {c_off} < 0")
+    _rows_view(out, B * T * H * W, c_off + Cc, "ncthw_to_rows.out")
     check(_lib.load().vc_ncthw_f32_to_rows_f16(x.data_ptr(), out.data_ptr(), B, Cc, T, H * W, c_off, out.stride(0), _stream()),
           "vc_ncthw_f32_to_rows_f16")
 
 
 def rows_to_ncthw(x: torch.Tensor, B: int, Cc: int, T: int, H: int, W: int) -> torch.Tensor:
-    assert x.dtype == torch.float32
+    """The first Cc columns of fp32 rows [(B T H W), >= Cc] -> [B,C,T,H,W]."""
+    if x.dtype != torch.float32 or not x.is_cuda:
+        raise VcError(f"rows_to_ncthw.x: expected a CUDA fp32 tensor, got {x.dtype} on {x.device}")
+    _rows_view(x, B * T * H * W, Cc, "rows_to_ncthw.x")
     out = torch.empty((B, Cc, T, H, W), device=x.device, dtype=torch.float32)
     check(_lib.load().vc_rows_f32_to_ncthw(x.data_ptr(), x.stride(0), out.data_ptr(), B, Cc, T, H * W, _stream()),
           "vc_rows_f32_to_ncthw")
@@ -655,7 +678,9 @@ def rows_to_ncthw(x: torch.Tensor, B: int, Cc: int, T: int, H: int, W: int) -> t
 
 
 def rows_f16_to_nchw(x: torch.Tensor, N: int, Cc: int, H: int, W: int) -> torch.Tensor:
+    """The first Cc columns of fp16 rows [(N H W), >= Cc] -> fp32 [N,C,H,W]."""
     _chk16(x, "rows_f16_to_nchw.x")
+    _rows_view(x, N * H * W, Cc, "rows_f16_to_nchw.x")
     out = torch.empty((N, Cc, H, W), device=x.device, dtype=torch.float32)
     check(_lib.load().vc_rows_f16_to_nchw_f32(x.data_ptr(), x.stride(0), out.data_ptr(), N, Cc, H * W, _stream()),
           "vc_rows_f16_to_nchw_f32")
@@ -670,6 +695,12 @@ def cast_f16(x: torch.Tensor) -> torch.Tensor:
 
 
 def add_f16(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+    """a + b of two contiguous fp16 tensors of one shape and an even element count (the kernel reads half2 pairs)."""
+    _chk16(a, "add.a")
+    _chk16(b, "add.b")
+    if a.shape != b.shape or not (a.is_contiguous() and b.is_contiguous()) or a.numel() % 2 or (a.data_ptr() | b.data_ptr()) % 4:
+        raise VcError(f"add_f16: expected two contiguous, 4-byte aligned fp16 tensors of one shape with an even element count, got "
+                      f"{tuple(a.shape)} and {tuple(b.shape)}")
     out = torch.empty_like(a)
     check(_lib.load().vc_add_f16(a.data_ptr(), b.data_ptr(), out.data_ptr(), a.numel(), _stream()), "vc_add_f16")
     return out
