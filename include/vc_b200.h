@@ -217,6 +217,14 @@ int vc_ddim_update3(const float* x, const float* v_cond, const float* v_uncond, 
 int vc_dpm_update(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img,
                   const float* noise, float* x0_hist, float* x_prev, float* pred_x0, int64_t n, const vc_ddim_scalars* s, float c_hist,
                   void* ws /* 4 * 1025 doubles */, void* stream);
+/* DPM-Solver++(3M) SDE step (eta = 1; INTEGRATION.md "Samplers"): vc_dpm_update's x_ddim, then
+ * x_prev = x_ddim + c1 (x0 - x0_hist1) + c2 (x0_hist1 - x0_hist2), x0_hist1 / x0_hist2 (n floats each) the x0 of the previous step and
+ * of the one before.  x0_hist1 is only read; x0_hist2 is overwritten with this step's x0, so the caller swaps the two buffers' roles
+ * after each step.  A zero coefficient reads nothing for its term; c2 = 0 gives vc_dpm_update's x_prev bit for bit.
+ * New functionality (the reference has only DDIM). */
+int vc_dpm3_update(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img,
+                   const float* noise, const float* x0_hist1, float* x0_hist2, float* x_prev, float* pred_x0, int64_t n,
+                   const vc_ddim_scalars* s, float c1, float c2, void* ws /* 4 * 1025 doubles */, void* stream);
 
 /* ---- multi-GPU: frame <-> site layout exchange over NVLink peer memory ------------------------------------------------
  * New functionality (the reference is single-GPU, SURVEY.md 8e).  The frame-sharded U-Net runs its spatial ops on

@@ -1,11 +1,12 @@
 #!/usr/bin/env python
-"""DPM-Solver++(2M) against DDIM on the full-width U-Net at 576x1024 x 25 frames, one GPU.
+"""DPM-Solver++(2M) and (3M) SDE against DDIM on the full-width U-Net at 576x1024 x 25 frames, one GPU.
 
-    python tools/bench_dpm.py [--dpm-steps 15,20,25] [--ode-steps 10,20,25,50] [--ode-ref-steps 200]
+    python tools/bench_dpm.py [--dpm-steps 15,20,25] [--dpm3-steps 8,10,15] [--ode-steps 10,20,25,50] [--ode-ref-steps 200]
 
-1. Seconds per clip, sampling + VAE decode: DDIM at --ddim-steps (50, the ViewCrafter default) and DPM-Solver++(2M) at each of
-   --dpm-steps.  Both run ViewCrafter's sampling settings: two-way CFG 7.5, guidance rescale 0.7, eta 1, uniform_trailing, batch_cfg
-   and graph replay.  Host clock around work that ends in a device synchronise, after one untimed warm-up of every stage.
+1. Seconds per clip, sampling + VAE decode: DDIM at --ddim-steps (50, the ViewCrafter default), DPM-Solver++(2M) at each of
+   --dpm-steps and DPM-Solver++(3M) SDE at each of --dpm3-steps.  All run ViewCrafter's sampling settings: two-way CFG 7.5, guidance
+   rescale 0.7, eta 1, uniform_trailing, batch_cfg and graph replay.  Host clock around work that ends in a device synchronise, after
+   one untimed warm-up of every stage.
 2. The ODE convergence of the real U-Net (eta 0, same guidance): the error of DDIM and DPM-Solver++(2M) at each of --ode-steps against
    a DPM-Solver++(2M) run of --ode-ref-steps from the same x_T, as max |diff| and RMS / RMS of the reference.
 
@@ -32,6 +33,7 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("--ddim-steps", type=int, default=50)
     ap.add_argument("--dpm-steps", default="15,20,25")
+    ap.add_argument("--dpm3-steps", default="8,10,15")
     ap.add_argument("--ode-steps", default="10,20,25,50", help="empty: skip the convergence table")
     ap.add_argument("--ode-ref-steps", type=int, default=200)
     args = ap.parse_args()
@@ -40,7 +42,7 @@ def main():
     from viewcrafter_b200.autoencoder import AutoencoderKL
     from viewcrafter_b200.configs import VAE_DDCONFIG
     from viewcrafter_b200.ddim import DDIMSampler
-    from viewcrafter_b200.dpm_solver import DPMSolverSampler
+    from viewcrafter_b200.dpm_solver import DPMSolver3MSDESampler, DPMSolverSampler
 
     if not torch.cuda.is_available():
         raise SystemExit("bench_dpm.py: no CUDA device")
@@ -80,9 +82,12 @@ def main():
     torch.manual_seed(5)
     model.decode_first_stage(sample(DDIMSampler, 3, 1.0, dev["x_T"]))
     sample(DPMSolverSampler, 5, 1.0, dev["x_T"])
+    sample(DPMSolver3MSDESampler, 5, 1.0, dev["x_T"])
     timing = {f"ddim_{args.ddim_steps}": clip(DDIMSampler, args.ddim_steps)}
     for s in [int(v) for v in args.dpm_steps.split(",") if v]:
         timing[f"dpmpp_2m_{s}"] = clip(DPMSolverSampler, s)
+    for s in [int(v) for v in args.dpm3_steps.split(",") if v]:
+        timing[f"dpmpp_3m_sde_{s}"] = clip(DPMSolver3MSDESampler, s)
 
     ode = {}
     ode_steps = [int(v) for v in args.ode_steps.split(",") if v]
@@ -95,7 +100,7 @@ def main():
                 d = sample(cls, s, 0.0, x_T).double() - ref
                 ode[f"{name}_{s}"] = {"max_abs": float(d.abs().max()), "rel_rms": rms(d) / rms(ref)}
     name, power = card()
-    print(json.dumps({"metric": "DPM-Solver++(2M) vs DDIM", "workload": "ViewCrafter_25", "px": wl["px"], "frames": T,
+    print(json.dumps({"metric": "DPM-Solver++(2M) / (3M) SDE vs DDIM", "workload": "ViewCrafter_25", "px": wl["px"], "frames": T,
                       "settings": "CFG 7.5, guidance rescale 0.7, uniform_trailing, batch_cfg, graph replay; clip timing eta 1, ODE eta 0",
                       "seconds_per_clip": timing, "ode_reference": f"dpmpp_2m_{args.ode_ref_steps} from the same x_T", "ode_error": ode,
                       "card": name, "power_limit": power}), flush=True)

@@ -9,6 +9,8 @@ Drop-in classes (same names / constructor kwargs / state-dict keys as the refere
     viewcrafter_b200.synthesis.image_guided_synthesis / get_latent_z <- utils.diffusion_utils (same names)
 Added samplers (opt-in; DDIM stays the default):
     viewcrafter_b200.dpm_solver.DPMSolverSampler / DPMSolverSamplerMultiCond: DPM-Solver++(2M), image_guided_synthesis(sampler="dpmpp_2m")
+    viewcrafter_b200.dpm_solver.DPMSolver3MSDESampler / DPMSolver3MSDESamplerMultiCond: DPM-Solver++(3M) SDE (eta = 1),
+        image_guided_synthesis(sampler="dpmpp_3m_sde")
 All tensor work runs in libvc_b200.so (hand-written CUDA for sm_90a, C ABI in include/vc_b200.h).
 
 set_reproducible(on) / VC_REPRODUCIBLE=1: reproducible mode (bit-identical results across batching, GPU count and SM count).

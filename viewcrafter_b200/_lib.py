@@ -108,6 +108,7 @@ SIGNATURES = {
     "vc_ddim_update": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, C.POINTER(DdimScalars), _vp, _vp]),
     "vc_ddim_update3": (C.c_int, [_vp, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _i64, C.POINTER(DdimScalars), _vp, _vp]),
     "vc_dpm_update": (C.c_int, [_vp, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _vp, _i64, C.POINTER(DdimScalars), _f32, _vp, _vp]),
+    "vc_dpm3_update": (C.c_int, [_vp, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _vp, _vp, _i64, C.POINTER(DdimScalars), _f32, _f32, _vp, _vp]),
 }
 
 _lib = None

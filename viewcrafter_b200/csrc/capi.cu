@@ -178,6 +178,14 @@ int vc_dpm_update(const float* x, const float* v_cond, const float* v_uncond, co
   return dpm_update(x, v_cond, v_uncond, v_uncond_img, cfg_img, noise, x0_hist, x_prev, pred_x0, n, *s, c_hist,
                     reinterpret_cast<double*>(ws), ST(stream));
 }
+int vc_dpm3_update(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img,
+                   const float* noise, const float* x0_hist1, float* x0_hist2, float* x_prev, float* pred_x0, int64_t n,
+                   const vc_ddim_scalars* s, float c1, float c2, void* ws, void* stream) {
+  if (!s) { set_error("vc_dpm3_update: null scalars"); return VC_ERR_ARG; }
+  COUNT((s->use_cfg && s->guidance_rescale > 0.f) ? 2 : 1);
+  return dpm3_update(x, v_cond, v_uncond, v_uncond_img, cfg_img, noise, x0_hist1, x0_hist2, x_prev, pred_x0, n, *s, c1, c2,
+                     reinterpret_cast<double*>(ws), ST(stream));
+}
 
 /* vc_enable_peer_access / vc_peer_exchange / vc_peer_groupnorm_stats: peer.cu */
 

@@ -74,5 +74,10 @@ int ddim_update(const float* x, const float* v_cond, const float* v_uncond, cons
 int dpm_update(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img, const float* noise,
                float* x0_hist, float* x_prev, float* pred_x0, long long n, const vc_ddim_scalars& s, float c_hist, double* ws,
                cudaStream_t stream);
+// ddim_update plus the DPM-Solver++(3M) SDE correction x_prev += c1 (x0 - x0_hist1) + c2 (x0_hist1 - x0_hist2), x0_hist1 / x0_hist2 the
+// previous two steps' x0; x0_hist1 is only read, x0_hist2 <- this step's x0 (before the dynamic rescale).  c2 = 0 is dpm_update bit for bit
+int dpm3_update(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img, const float* noise,
+                const float* x0_hist1, float* x0_hist2, float* x_prev, float* pred_x0, long long n, const vc_ddim_scalars& s, float c1,
+                float c2, double* ws, cudaStream_t stream);
 
 }  // namespace vc

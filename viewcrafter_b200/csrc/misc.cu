@@ -354,15 +354,22 @@ int ddim_update(const float* x, const float* v_cond, const float* v_uncond, cons
 }
 
 // ------------------------------------------------------------------------------------------------
-// DPM-Solver++(2M) update (INTEGRATION.md "Samplers"): the DDIM step above, x_ddim, plus the multistep correction
-//   x_prev = x_ddim + c_hist (x0 - x0_hist),   x0 = sqrt_ac_t x - sqrt_1mac_t v  (before the dynamic rescale)
-// x0_hist holds the previous step's x0 and is overwritten with this step's.  c_hist = 0 is a first-order step: x_prev is x_ddim
-// bit for bit and x0_hist is not read (it may be uninitialised on the first step).  x_ddim is ddim_apply_kernel's expression.
+// DPM-Solver++ multistep updates (INTEGRATION.md "Samplers"): the DDIM step above, x_ddim, plus the multistep correction
+//   NH = 1, 2M:      x_prev = x_ddim + c_hist (x0 - m1)
+//   NH = 2, 3M SDE:  x_prev = x_ddim + c_hist (x0 - m1) + c_hist2 (m1 - m2)
+// with x0 = sqrt_ac_t x - sqrt_1mac_t v (before the dynamic rescale), m1 / m2 the x0 of the previous step / the one before.
+// NH = 1: x0_hist holds m1 and is overwritten with this step's x0.  NH = 2: x0_hist holds m2 and is overwritten with this step's
+// x0; x0_hist1 holds m1 and is only read.  A zero coefficient reads nothing for its term (a history may be uninitialised), and each
+// non-zero one is one more __fmaf_rn: c_hist = c_hist2 = 0 is x_ddim bit for bit, c_hist2 = 0 is the NH = 1 update bit for bit.
+// x_ddim is ddim_apply_kernel's expression.
 // ------------------------------------------------------------------------------------------------
+template <int NH>
 __global__ void dpm_apply_kernel(const float* __restrict__ x, const float* __restrict__ vc_, const float* __restrict__ vu,
                                  const float* __restrict__ vi, float cfg_img,
-                                 const float* __restrict__ noise, float* __restrict__ x0_hist, float* __restrict__ x_prev,
-                                 float* __restrict__ pred_x0, long long n, vc_ddim_scalars s, float c_hist, const double* ws, int stat_blocks) {
+                                 const float* __restrict__ noise, const float* __restrict__ x0_hist1, float* __restrict__ x0_hist,
+                                 float* __restrict__ x_prev, float* __restrict__ pred_x0, long long n, vc_ddim_scalars s, float c_hist,
+                                 float c_hist2, const double* ws, int stat_blocks) {
+  static_assert(NH == 1 || NH == 2, "dpm_apply_kernel: one or two x0 histories");
   float factor = 1.f;
   if (s.use_cfg && s.guidance_rescale > 0.f) {
     __shared__ double tot[4];
@@ -397,9 +404,36 @@ __global__ void dpm_apply_kernel(const float* __restrict__ x, const float* __res
     p0 *= rescale;
     pred_x0[i] = p0;
     const float x_ddim = sq_ap * p0 + dir_c * e_t + s.sigma_t * noise[i];
-    x_prev[i] = c_hist != 0.f ? __fmaf_rn(c_hist, x0 - x0_hist[i], x_ddim) : x_ddim;
+    if (NH == 1) {
+      x_prev[i] = c_hist != 0.f ? __fmaf_rn(c_hist, x0 - x0_hist[i], x_ddim) : x_ddim;
+    } else {
+      const float m1 = (c_hist != 0.f || c_hist2 != 0.f) ? x0_hist1[i] : 0.f;
+      float xp = c_hist != 0.f ? __fmaf_rn(c_hist, x0 - m1, x_ddim) : x_ddim;
+      if (c_hist2 != 0.f) xp = __fmaf_rn(c_hist2, m1 - x0_hist[i], xp);
+      x_prev[i] = xp;
+    }
     x0_hist[i] = x0;
   }
+}
+// x0_hist1 == nullptr: the NH = 1 kernel (c_hist2 unused)
+static int dpm_launch(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img,
+                      const float* noise, const float* x0_hist1, float* x0_hist, float* x_prev, float* pred_x0, long long n,
+                      const vc_ddim_scalars& s, float c_hist, float c_hist2, double* ws, cudaStream_t stream) {
+  // the statistics grid of ddim_update (reproducible mode included), so every update reduces the same partial sums in the same order
+  int blocks = (int)min(s.reproducible ? (long long)DDIM_REPRO_BLOCKS : (long long)sm_count() * 4, (n + 255) / 256);
+  if (blocks > DDIM_MAX_BLOCKS) blocks = DDIM_MAX_BLOCKS;
+  if (s.use_cfg && s.guidance_rescale > 0.f) {
+    ddim_stats_kernel<<<blocks, 256, 0, stream>>>(v_cond, v_uncond, v_uncond_img, n, s.cfg_scale, cfg_img, ws);
+    VC_CHECK_CUDA(cudaGetLastError());
+  }
+  if (x0_hist1 == nullptr)
+    dpm_apply_kernel<1><<<blocks, 256, 0, stream>>>(x, v_cond, v_uncond, v_uncond_img, cfg_img, noise, nullptr, x0_hist, x_prev, pred_x0,
+                                                    n, s, c_hist, 0.f, ws, blocks);
+  else
+    dpm_apply_kernel<2><<<blocks, 256, 0, stream>>>(x, v_cond, v_uncond, v_uncond_img, cfg_img, noise, x0_hist1, x0_hist, x_prev, pred_x0,
+                                                    n, s, c_hist, c_hist2, ws, blocks);
+  VC_CHECK_CUDA(cudaGetLastError());
+  return VC_OK;
 }
 int dpm_update(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img, const float* noise,
                float* x0_hist, float* x_prev, float* pred_x0, long long n, const vc_ddim_scalars& s, float c_hist, double* ws,
@@ -409,17 +443,18 @@ int dpm_update(const float* x, const float* v_cond, const float* v_uncond, const
   VC_REQUIRE(!v_uncond_img || s.use_cfg, "dpm_update: the image-only branch is only defined with CFG on");
   VC_REQUIRE(x0_hist != x_prev && x0_hist != pred_x0 && x0_hist != x && x_prev != pred_x0, "dpm_update: x0_hist, x_prev and pred_x0 must not alias");
   VC_REQUIRE(isfinite(c_hist), "dpm_update: c_hist must be finite");
-  // the statistics grid of ddim_update (reproducible mode included), so both updates reduce the same partial sums in the same order
-  int blocks = (int)min(s.reproducible ? (long long)DDIM_REPRO_BLOCKS : (long long)sm_count() * 4, (n + 255) / 256);
-  if (blocks > DDIM_MAX_BLOCKS) blocks = DDIM_MAX_BLOCKS;
-  if (s.use_cfg && s.guidance_rescale > 0.f) {
-    ddim_stats_kernel<<<blocks, 256, 0, stream>>>(v_cond, v_uncond, v_uncond_img, n, s.cfg_scale, cfg_img, ws);
-    VC_CHECK_CUDA(cudaGetLastError());
-  }
-  dpm_apply_kernel<<<blocks, 256, 0, stream>>>(x, v_cond, v_uncond, v_uncond_img, cfg_img, noise, x0_hist, x_prev, pred_x0, n, s, c_hist,
-                                               ws, blocks);
-  VC_CHECK_CUDA(cudaGetLastError());
-  return VC_OK;
+  return dpm_launch(x, v_cond, v_uncond, v_uncond_img, cfg_img, noise, nullptr, x0_hist, x_prev, pred_x0, n, s, c_hist, 0.f, ws, stream);
+}
+int dpm3_update(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img, const float* noise,
+                const float* x0_hist1, float* x0_hist2, float* x_prev, float* pred_x0, long long n, const vc_ddim_scalars& s, float c1,
+                float c2, double* ws, cudaStream_t stream) {
+  VC_REQUIRE(x && v_cond && noise && x0_hist1 && x0_hist2 && x_prev && pred_x0 && ws && n > 1, "dpm3_update: bad args");
+  VC_REQUIRE(!s.use_cfg || v_uncond, "dpm3_update: CFG needs the unconditional output");
+  VC_REQUIRE(!v_uncond_img || s.use_cfg, "dpm3_update: the image-only branch is only defined with CFG on");
+  VC_REQUIRE(x0_hist1 != x0_hist2 && x0_hist1 != x_prev && x0_hist1 != pred_x0 && x0_hist2 != x_prev && x0_hist2 != pred_x0 &&
+             x0_hist2 != x && x_prev != pred_x0, "dpm3_update: x0_hist1, x0_hist2, x_prev and pred_x0 must not alias");
+  VC_REQUIRE(isfinite(c1) && isfinite(c2), "dpm3_update: c1 and c2 must be finite");
+  return dpm_launch(x, v_cond, v_uncond, v_uncond_img, cfg_img, noise, x0_hist1, x0_hist2, x_prev, pred_x0, n, s, c1, c2, ws, stream);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -737,11 +737,9 @@ def small_linear(x: torch.Tensor, w: torch.Tensor, b: Optional[torch.Tensor], si
 _ddim_ws = {}
 
 
-def ddim_update(x, v_cond, v_uncond, noise, sc: dict, v_uncond_img=None, cfg_img: float = 0.0):
-    """Fused ddim.py:228-281.  sc: cfg_scale, guidance_rescale, sqrt_ac_t, sqrt_1mac_t, a_prev, sigma_t, scale_t, prev_scale_t.
-    v_uncond_img / cfg_img: the third ("image, no text") branch of ddim_multiplecond.py:227-233."""
-    for t in (x, v_cond, noise) + ((v_uncond_img,) if v_uncond_img is not None else ()):
-        assert t.dtype == torch.float32 and t.is_contiguous() and t.is_cuda
+def _update_args(x, v_uncond, sc: dict):
+    """(vc_ddim_scalars, use_cfg, workspace) of one fused DDIM / DPM-Solver update: the step scalars `sc`, and the per-(device, stream)
+    buffer of the per-block partial sums of the two std reductions."""
     s = DdimScalars()
     use_cfg = v_uncond is not None and sc["cfg_scale"] != 1.0
     s.cfg_scale, s.guidance_rescale = sc["cfg_scale"], sc["guidance_rescale"] if use_cfg else 0.0
@@ -752,8 +750,17 @@ def ddim_update(x, v_cond, v_uncond, noise, sc: dict, v_uncond_img=None, cfg_img
     key = (x.device, torch.cuda.current_stream().cuda_stream)
     ws = _ddim_ws.get(key)
     if ws is None:
-        ws = torch.zeros(4 * 1025, device=x.device, dtype=torch.float64)    # per-block partial sums of the two std reductions
+        ws = torch.zeros(4 * 1025, device=x.device, dtype=torch.float64)
         _ddim_ws[key] = ws
+    return s, use_cfg, ws
+
+
+def ddim_update(x, v_cond, v_uncond, noise, sc: dict, v_uncond_img=None, cfg_img: float = 0.0):
+    """Fused ddim.py:228-281.  sc: cfg_scale, guidance_rescale, sqrt_ac_t, sqrt_1mac_t, a_prev, sigma_t, scale_t, prev_scale_t.
+    v_uncond_img / cfg_img: the third ("image, no text") branch of ddim_multiplecond.py:227-233."""
+    for t in (x, v_cond, noise) + ((v_uncond_img,) if v_uncond_img is not None else ()):
+        assert t.dtype == torch.float32 and t.is_contiguous() and t.is_cuda
+    s, use_cfg, ws = _update_args(x, v_uncond, sc)
     x_prev, pred_x0 = torch.empty_like(x), torch.empty_like(x)
     if v_uncond_img is not None and use_cfg:
         check(_lib.load().vc_ddim_update3(x.data_ptr(), v_cond.data_ptr(), v_uncond.data_ptr(), v_uncond_img.data_ptr(), float(cfg_img),
@@ -773,21 +780,28 @@ def dpm_update(x, v_cond, v_uncond, noise, sc: dict, x0_hist, v_uncond_img=None,
     for t in (x, v_cond, noise, x0_hist) + ((v_uncond_img,) if v_uncond_img is not None else ()):
         assert t.dtype == torch.float32 and t.is_contiguous() and t.is_cuda
     assert x0_hist.shape == x.shape
-    s = DdimScalars()
-    use_cfg = v_uncond is not None and sc["cfg_scale"] != 1.0
-    s.cfg_scale, s.guidance_rescale = sc["cfg_scale"], sc["guidance_rescale"] if use_cfg else 0.0
-    s.sqrt_ac_t, s.sqrt_1mac_t = sc["sqrt_ac_t"], sc["sqrt_1mac_t"]
-    s.a_prev, s.sigma_t, s.scale_t, s.prev_scale_t = sc["a_prev"], sc["sigma_t"], sc["scale_t"], sc["prev_scale_t"]
-    s.use_cfg = int(use_cfg)
-    s.reproducible = int(REPRODUCIBLE)
-    key = (x.device, torch.cuda.current_stream().cuda_stream)
-    ws = _ddim_ws.get(key)
-    if ws is None:
-        ws = torch.zeros(4 * 1025, device=x.device, dtype=torch.float64)
-        _ddim_ws[key] = ws
+    s, use_cfg, ws = _update_args(x, v_uncond, sc)
     x_prev, pred_x0 = torch.empty_like(x), torch.empty_like(x)
     vi = v_uncond_img if use_cfg else None
     check(_lib.load().vc_dpm_update(x.data_ptr(), v_cond.data_ptr(), _ptr(v_uncond) if use_cfg else None, _ptr(vi), float(cfg_img),
                                     noise.data_ptr(), x0_hist.data_ptr(), x_prev.data_ptr(), pred_x0.data_ptr(), x.numel(), C.byref(s),
                                     float(sc["c_hist"]), ws.data_ptr(), _stream()), "vc_dpm_update")
+    return x_prev, pred_x0
+
+
+def dpm3_update(x, v_cond, v_uncond, noise, sc: dict, x0_hist1, x0_hist2, v_uncond_img=None, cfg_img: float = 0.0):
+    """One DPM-Solver++(3M) SDE step (vc_dpm3_update): ddim_update's x_{t-1} (eta = 1), plus sc["c1"] * (x0 - x0_hist1) +
+    sc["c2"] * (x0_hist1 - x0_hist2), where x0 is this step's x0 prediction before the dynamic rescale.  x0_hist1 / x0_hist2 (fp32,
+    x's shape) hold the previous step's x0 and the one before; a term whose coefficient is 0 reads nothing.  x0_hist1 is only read and
+    x0_hist2 is overwritten in place with this step's x0, so the caller swaps the two after each step.  sc["c2"] = 0 gives dpm_update's
+    x_prev with c_hist = sc["c1"] bit for bit.  Returns (x_prev, pred_x0) like ddim_update."""
+    for t in (x, v_cond, noise, x0_hist1, x0_hist2) + ((v_uncond_img,) if v_uncond_img is not None else ()):
+        assert t.dtype == torch.float32 and t.is_contiguous() and t.is_cuda
+    assert x0_hist1.shape == x.shape and x0_hist2.shape == x.shape
+    s, use_cfg, ws = _update_args(x, v_uncond, sc)
+    x_prev, pred_x0 = torch.empty_like(x), torch.empty_like(x)
+    vi = v_uncond_img if use_cfg else None
+    check(_lib.load().vc_dpm3_update(x.data_ptr(), v_cond.data_ptr(), _ptr(v_uncond) if use_cfg else None, _ptr(vi), float(cfg_img),
+                                     noise.data_ptr(), x0_hist1.data_ptr(), x0_hist2.data_ptr(), x_prev.data_ptr(), pred_x0.data_ptr(),
+                                     x.numel(), C.byref(s), float(sc["c1"]), float(sc["c2"]), ws.data_ptr(), _stream()), "vc_dpm3_update")
     return x_prev, pred_x0

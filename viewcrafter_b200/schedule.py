@@ -74,6 +74,32 @@ def dpm_coefficients(alphacums, ts: np.ndarray, eta: float) -> np.ndarray:
     return c
 
 
+def dpm3_coefficients(alphacums, ts: np.ndarray):
+    """float64 ([S], [S]): (c1, c2) of the DPM-Solver++(3M) SDE step (eta = 1) of DDIM index j (INTEGRATION.md "Samplers"), with a, a',
+    lambda and h_j as in dpm_coefficients, h_e = 2 h_j, r0 = h_{j+1} / h_j and r1 = h_{j+2} / h_j:
+        phi2 = expm1(-h_e) / h_e + 1,   phi3 = phi2 / h_e - 1/2
+        c1_j = sqrt(a') [phi2 (1 + r0 / (r0 + r1)) - phi3 / (r0 + r1)] / r0,   c2_j = sqrt(a') [phi3 / (r0 + r1) - phi2 r0 / (r0 + r1)] / r1
+    Fallbacks: c1 = c2 = 0 (first order) wherever dpm_coefficients(..., eta=1) is 0; otherwise, where h_{j+2} is infinite (step j + 2
+    started at a = 0), zero or absent (j + 2 = S), c2 = 0 and c1 is dpm_coefficients' c exactly (the 2M step)."""
+    ac = np.asarray(alphacums, dtype=np.float64)
+    a = ac[ts]
+    a_prev = np.concatenate([ac[0:1], a[:-1]])
+    with np.errstate(divide="ignore"):
+        lam = lambda v: 0.5 * (np.log(v) - np.log1p(-v))
+        h = lam(a_prev) - lam(a)
+    c1 = dpm_coefficients(ac, ts, 1.0)
+    c2 = np.zeros(len(ts), dtype=np.float64)
+    for j in range(1, len(ts) - 2):
+        if c1[j] != 0 and np.isfinite(h[j + 2]) and h[j + 2] != 0:
+            he = 2.0 * h[j]
+            r0, r1 = h[j + 1] / h[j], h[j + 2] / h[j]
+            phi2 = np.expm1(-he) / he + 1.0
+            phi3 = phi2 / he - 0.5
+            c1[j] = np.sqrt(a_prev[j]) * (phi2 * (1.0 + r0 / (r0 + r1)) - phi3 / (r0 + r1)) / r0
+            c2[j] = np.sqrt(a_prev[j]) * (phi3 / (r0 + r1) - phi2 * r0 / (r0 + r1)) / r1
+    return c1, c2
+
+
 def f32(v) -> float:
     """The value torch.full(size, v) would hold (float32 rounding of a python/numpy/tensor scalar)."""
     return float(np.float32(float(v)))

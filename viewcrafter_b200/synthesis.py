@@ -26,10 +26,11 @@ import torch
 from . import ops, parallel
 from .ddim import DDIMSampler, check_row_replay
 from .ddim_multiplecond import DDIMSampler as DDIMSampler_multicond
-from .dpm_solver import DPMSolverSampler, DPMSolverSamplerMultiCond, check_eta
+from .dpm_solver import DPMSolver3MSDESampler, DPMSolver3MSDESamplerMultiCond, DPMSolverSampler, DPMSolverSamplerMultiCond
 
 # image_guided_synthesis(sampler=...) -> (two-way sampler class, three-way sampler class)
-SAMPLERS = {"ddim": (DDIMSampler, DDIMSampler_multicond), "dpmpp_2m": (DPMSolverSampler, DPMSolverSamplerMultiCond)}
+SAMPLERS = {"ddim": (DDIMSampler, DDIMSampler_multicond), "dpmpp_2m": (DPMSolverSampler, DPMSolverSamplerMultiCond),
+            "dpmpp_3m_sde": (DPMSolver3MSDESampler, DPMSolver3MSDESamplerMultiCond)}
 
 
 def _vae_sharded(model) -> bool:
@@ -55,12 +56,13 @@ def image_guided_synthesis(model, prompts, videos, noise_shape, n_samples=1, ddi
                            reproducible=None, sampler="ddim", **kwargs):
     """reproducible: True / False switches viewcrafter_b200's reproducible mode (ops.set_reproducible) for this call and restores the
     previous setting afterwards; None leaves the process setting as it is.
-    sampler: "ddim" (the reference's DDIMSampler) or "dpmpp_2m" (dpm_solver.DPMSolverSampler / DPMSolverSamplerMultiCond, which takes
-    ddim_eta 0 or 1 only; INTEGRATION.md "Samplers")."""
+    sampler: "ddim" (the reference's DDIMSampler), "dpmpp_2m" (dpm_solver.DPMSolverSampler / DPMSolverSamplerMultiCond, which takes
+    ddim_eta 0 or 1 only) or "dpmpp_3m_sde" (dpm_solver.DPMSolver3MSDESampler / DPMSolver3MSDESamplerMultiCond, ddim_eta 1 only;
+    INTEGRATION.md "Samplers")."""
     if sampler not in SAMPLERS:
         raise ValueError(f"unknown sampler {sampler!r}; choose one of {sorted(SAMPLERS)}")
-    if sampler == "dpmpp_2m":
-        check_eta(ddim_eta)                               # before the conditioning is computed
+    if sampler != "ddim":
+        SAMPLERS[sampler][0].check_eta(ddim_eta)          # before the conditioning is computed
     if reproducible is None:
         return _synthesis(model, prompts, videos, noise_shape, n_samples, ddim_steps, ddim_eta, unconditional_guidance_scale, cfg_img, fs,
                           text_input, multiple_cond_cfg, timestep_spacing, guidance_rescale, condition_index, batch_cfg, cuda_graph,
