@@ -116,6 +116,11 @@ int vc_flash_attn_d64(const vc_attn_desc* d, void* stream);
  * always the naive path in the reference, attention.py:66).  q/k/v rows at (t*sites + site), pitch ld. */
 int vc_temporal_attn(const void* q, const void* k, const void* v, int32_t ld, void* out, int32_t ldo, int32_t T,
                      int64_t sites, int32_t heads, float scale, void* stream);
+/* windowed temporal self-attention (FreeNoise): softmax attention over windows of 2 <= W <= 32 frames at starts 0, S, 2S, ...
+ * (while start + W < T) plus T - W, 1 <= S <= W; out_t is the mean of the windows' outputs for frame t weighted by
+ * min(j + 1, W - j) (j = frame index in the window).  Any T >= 1; T <= W is vc_temporal_attn.  Same row layout as vc_temporal_attn. */
+int vc_temporal_attn_windowed(const void* q, const void* k, const void* v, int32_t ld, void* out, int32_t ldo, int32_t T,
+                              int64_t sites, int32_t heads, int32_t W, int32_t S, float scale, void* stream);
 
 /* ---- normalisation --------------------------------------------------------------------------------------------
  * GroupNorm(32)+optional SiLU on channels-last fp16; x = concat(x1[C1], x2[C2]) along channels (x2 may be NULL).

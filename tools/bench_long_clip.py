@@ -17,6 +17,14 @@ temporal-attention kernel alone.
    kernel) and T = 49 (the long-clip kernel) in the same run: device time per call over --reps launches (CUDA events) and the rate of
    its algorithmic bytes, 4 * B * T * sites * heads * 64 * 2 (q, k, v read once, out written once).
 Prints one JSON line with every number, the card name and its power limit.
+
+    python tools/bench_long_clip.py --window W,S [--frames 49,128] [--steps 3] [--warmup 2] [--reps 50]
+
+runs the windowed temporal attention (UNetModel.set_temporal_window) instead: two-way steps/s and peak memory for every T of --frames
+with the window and, where full attention exists (T <= 128), without it.  A configuration that runs out of device memory is recorded
+as such (with the allocator's message) and the remaining ones still run; then the kernel alone at level 0 (B = 2) for T = 49 and 128,
+windowed against the full kernels, with the algorithmic bytes 4 * T * 128 per (site, head) pair (each q, k, v row read once, each
+output row written once).
 """
 from __future__ import annotations
 
@@ -78,7 +86,7 @@ def time_steps(model, B, T, steps, warmup):
     return rate, peak, finite
 
 
-def kernel_rate(B, T, sites, heads, reps):
+def kernel_rate(B, T, sites, heads, reps, window=None):
     from viewcrafter_b200 import ops
     C = heads * 64
     g = torch.Generator(device="cuda").manual_seed(T)
@@ -88,7 +96,10 @@ def kernel_rate(B, T, sites, heads, reps):
     def call():
         for b in range(B):                             # the U-Net's call sequence: one launch per batch element
             rows = slice(b * T * sites, (b + 1) * T * sites)
-            ops.temporal_attn(qkv[rows, :C], qkv[rows, C:2 * C], qkv[rows, 2 * C:], T, sites, heads, out=a[rows])
+            if window is None:
+                ops.temporal_attn(qkv[rows, :C], qkv[rows, C:2 * C], qkv[rows, 2 * C:], T, sites, heads, out=a[rows])
+            else:
+                ops.temporal_attn_windowed(qkv[rows, :C], qkv[rows, C:2 * C], qkv[rows, 2 * C:], T, sites, heads, *window, out=a[rows])
 
     for _ in range(5):
         call()
@@ -101,24 +112,65 @@ def kernel_rate(B, T, sites, heads, reps):
     torch.cuda.synchronize()
     dt = e0.elapsed_time(e1) * 1e-3 / reps
     nbytes = 4 * B * T * sites * heads * 64 * 2
-    return dict(level_sites=sites, heads=heads, B=B, T=T, kernel="T<=32" if T <= 32 else "33..128", us=round(dt * 1e6, 2),
-                GB_per_s=round(nbytes / dt / 1e9, 1), bytes=nbytes)
+    kernel = f"windowed{tuple(window)}" if window is not None else "T<=32" if T <= 32 else "33..128"
+    return dict(level_sites=sites, heads=heads, B=B, T=T, kernel=kernel, us=round(dt * 1e6, 2), GB_per_s=round(nbytes / dt / 1e9, 1),
+                bytes=nbytes)
+
+
+def window_main(args, window):
+    import bench
+    from bench_multicond import card
+    torch.cuda.set_device(0)
+    frames = sorted(int(t) for t in (args.frames or "49,128").split(","))
+    res = {"metric": f"windowed temporal attention {window} at 576x1024 (1 GPU, two-way batch_cfg, graph replay)", "kernel": []}
+    for T in (49, 128):
+        for w in (None, window):
+            res["kernel"].append(kernel_rate(2, T, H * W, 5, args.reps, w))
+            print(json.dumps(res["kernel"][-1]), flush=True)
+    torch.cuda.empty_cache()
+    model = bench.build_model(bench.WORKLOADS["ViewCrafter_25"], torch.device("cuda"))
+    unet = model.model.diffusion_model
+    runs = []
+    for T in frames:
+        for w in ((None, window) if T <= MAX_T else (window,)):
+            unet.set_temporal_window(w)
+            oom = None
+            try:
+                rate, peak, finite = time_steps(model, 2, T, args.steps, args.warmup)
+            except torch.OutOfMemoryError as e:
+                oom = ". ".join(str(e).split(". ")[:2]) + "."       # "CUDA out of memory. Tried to allocate ..."
+            if oom is None:
+                runs.append(dict(B=2, T=T, window=w, steps_per_s=round(rate, 4), peak_GB=round(peak / 1e9, 2), finite=finite))
+            else:                                          # the exception and its frames are gone: release the graphs and the cache
+                unet.enable_cuda_graph(False)
+                torch.cuda.empty_cache()
+                runs.append(dict(B=2, T=T, window=w, out_of_memory=oom, peak_GB=round(torch.cuda.max_memory_allocated() / 1e9, 2)))
+            print(json.dumps(runs[-1]), flush=True)
+    unet.set_temporal_window(None)
+    res["runs"] = runs
+    name, power = card()
+    res.update(card=name, power_limit=power)
+    print(json.dumps(res), flush=True)
 
 
 def main():
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
-    ap.add_argument("--frames", default="25,49,64,96")
+    ap.add_argument("--frames", default=None, help="default 25,49,64,96 (49,128 with --window)")
     ap.add_argument("--steps", type=int, default=5, help="timed DDIM steps per configuration")
     ap.add_argument("--warmup", type=int, default=2, help="untimed steps first (eager, capture)")
     ap.add_argument("--reps", type=int, default=200, help="temporal_attn launches per kernel timing")
+    ap.add_argument("--window", default=None, help="W,S: measure windowed temporal attention instead")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_long_clip.py: no CUDA device")
+    if args.window is not None:
+        from viewcrafter_b200.temporal_window import check_window
+        return window_main(args, check_window(tuple(int(v) for v in args.window.split(","))))
     import bench
     from bench_multicond import card
 
     torch.cuda.set_device(0)
-    frames = sorted(int(t) for t in args.frames.split(","))
+    frames = sorted(int(t) for t in (args.frames or "25,49,64,96").split(","))
     res = {"metric": "long clips at 576x1024 (1 GPU, batch_cfg, graph replay)", "kernel": []}
     # kernel first, while the card holds nothing else of ours
     for sites, heads in ((H * W, 5), (H * W // 4, 10)):

@@ -71,6 +71,7 @@ SIGNATURES = {
     "vc_absmax_f16": (C.c_int, [_vp, _i64, _i32, _i32, _vp, _i32, _i32, _vp, _vp]),
     "vc_flash_attn_d64": (C.c_int, [C.POINTER(AttnDesc), _vp]),
     "vc_temporal_attn": (C.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _i32, _i64, _i32, _f32, _vp]),
+    "vc_temporal_attn_windowed": (C.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _i32, _i64, _i32, _i32, _i32, _f32, _vp]),
     "vc_groupnorm_ws_bytes": (_sz, [_i32]),
     "vc_groupnorm_nhwc": (C.c_int, [_vp, _i32, _vp, _i32, _i32, _i64, _vp, _vp, _f32, _i32, _vp, _vp, _sz, _vp]),
     "vc_groupnorm_stats": (C.c_int, [_vp, _i32, _vp, _i32, _i32, _i64, _vp, _vp, _sz, _vp]),

@@ -48,6 +48,12 @@ int vc_temporal_attn(const void* q, const void* k, const void* v, int32_t ld, vo
   return temporal_attn(H(q), H(k), H(v), ld, HM(out), ldo, T, sites, heads, scale, ST(stream));
 }
 
+int vc_temporal_attn_windowed(const void* q, const void* k, const void* v, int32_t ld, void* out, int32_t ldo, int32_t T,
+                              int64_t sites, int32_t heads, int32_t W, int32_t S, float scale, void* stream) {
+  COUNT(1);
+  return temporal_attn_windowed(H(q), H(k), H(v), ld, HM(out), ldo, T, sites, heads, W, S, scale, ST(stream));
+}
+
 size_t vc_groupnorm_ws_bytes(int32_t samples) { return groupnorm_ws_bytes(samples); }
 int vc_groupnorm_nhwc(const void* x1, int32_t C1, const void* x2, int32_t C2, int32_t samples, int64_t rows_per_sample,
                       const float* gamma, const float* beta, float eps, int32_t silu, void* out, void* ws, size_t ws_bytes,

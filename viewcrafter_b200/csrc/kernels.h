@@ -51,6 +51,10 @@ int layernorm_rows(const __half* x, long long rows, int C, const float* gamma, c
 // [T*sites, ld] with q|k|v at column offsets.
 int temporal_attn(const __half* q, const __half* k, const __half* v, int ld, __half* out, int ldo, int T, long long sites,
                   int heads, float scale, cudaStream_t stream);
+// The same attention on overlapping windows of W frames with stride S, blended per frame (vc_temporal_attn_windowed); T <= W
+// runs temporal_attn.
+int temporal_attn_windowed(const __half* q, const __half* k, const __half* v, int ld, __half* out, int ldo, int T, long long sites,
+                           int heads, int W, int S, float scale, cudaStream_t stream);
 
 int upsample2x_nhwc(const __half* x, __half* out, int N, int H, int W, int C, cudaStream_t stream);
 int im2col3x3_s2_nhwc(const __half* x, __half* out, int N, int H, int W, int C, int pad_lo, int Ho, int Wo, cudaStream_t stream);

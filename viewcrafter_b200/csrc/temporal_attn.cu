@@ -28,6 +28,112 @@ __device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], 
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
+// One warp's 32 x 32 x 64 attention tile: S = Q K^T, softmax over the first n keys (n <= 32; keys >= n are masked, so their K
+// rows may hold any finite value and their V rows must be finite), O = P V.  rows.q(r) / rows.k(r) / rows.v(r) give the shared-memory
+// address of row r (64 halves, 16-byte aligned).  O (unnormalised) and 1/l are left in the mma accumulator layout: thread
+// (g = lane / 4, tg = lane % 4) holds rows mi * 16 + g (+ 8 for h = 1), columns ni * 8 + 2 * tg (+ 1).
+template <class Rows>
+__device__ __forceinline__ void ta_tile32(const Rows& rows, int n, float scale_log2, int lane, float (&o)[2][8][4], float (&inv_l)[2][2]) {
+  const int tg = lane & 3;
+  // ---- S = Q K^T : [32 x 32], k = 64 ----
+  float s[2][4][4];
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+    for (int ni = 0; ni < 4; ++ni)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) s[mi][ni][e] = 0.f;
+  const int mat = lane >> 3, mr = lane & 7;
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) {
+    uint32_t a[2][4];
+#pragma unroll
+    for (int mi = 0; mi < 2; ++mi)
+      ldsm_x4(a[mi][0], a[mi][1], a[mi][2], a[mi][3], rows.q(mi * 16 + (mat & 1) * 8 + mr) + kk * 16 + (mat >> 1) * 8);
+#pragma unroll
+    for (int np = 0; np < 2; ++np) {                       // two n-tiles (16 keys) per ldmatrix.x4
+      uint32_t b0, b1, b2, b3;
+      ldsm_x4(b0, b1, b2, b3, rows.k(np * 16 + (mat >> 1) * 8 + mr) + kk * 16 + (mat & 1) * 8);
+#pragma unroll
+      for (int mi = 0; mi < 2; ++mi) {
+        mma16816(s[mi][2 * np], a[mi], b0, b1);
+        mma16816(s[mi][2 * np + 1], a[mi], b2, b3);
+      }
+    }
+  }
+
+  // ---- softmax over the key axis (columns); each thread owns rows g / g+8 of both m-tiles ----
+  uint32_t p[2][2][4];                                      // P as A fragments: [m-tile][k-step of 16 keys][4]
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {                           // h = 0: row g, h = 1: row g + 8
+      float mx = -INFINITY;
+#pragma unroll
+      for (int ni = 0; ni < 4; ++ni)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int col = ni * 8 + 2 * tg + e;
+          float val = s[mi][ni][2 * h + e];
+          if (col >= n) val = -INFINITY;
+          s[mi][ni][2 * h + e] = val;
+          mx = fmaxf(mx, val);
+        }
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float off = mx * scale_log2;
+      float l = 0.f;
+#pragma unroll
+      for (int ni = 0; ni < 4; ++ni)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float pv = exp2f(fmaf(s[mi][ni][2 * h + e], scale_log2, -off));
+          s[mi][ni][2 * h + e] = pv;
+          l += pv;
+        }
+      l += __shfl_xor_sync(0xffffffffu, l, 1);
+      l += __shfl_xor_sync(0xffffffffu, l, 2);
+      inv_l[mi][h] = 1.f / l;
+    }
+#pragma unroll
+    for (int kk = 0; kk < 2; ++kk) {
+      p[mi][kk][0] = pack_half2(s[mi][2 * kk][0], s[mi][2 * kk][1]);
+      p[mi][kk][1] = pack_half2(s[mi][2 * kk][2], s[mi][2 * kk][3]);
+      p[mi][kk][2] = pack_half2(s[mi][2 * kk + 1][0], s[mi][2 * kk + 1][1]);
+      p[mi][kk][3] = pack_half2(s[mi][2 * kk + 1][2], s[mi][2 * kk + 1][3]);
+    }
+  }
+
+  // ---- O = P V : [32 x 64], k = 32 keys ----
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+    for (int ni = 0; ni < 8; ++ni)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) o[mi][ni][e] = 0.f;
+#pragma unroll
+  for (int kk = 0; kk < 2; ++kk) {
+#pragma unroll
+    for (int np = 0; np < 4; ++np) {                       // two d-tiles (16 columns) per ldmatrix.x4.trans
+      uint32_t b0, b1, b2, b3;
+      ldsm_x4_t(b0, b1, b2, b3, rows.v(kk * 16 + (mat & 1) * 8 + mr) + np * 16 + (mat >> 1) * 8);
+#pragma unroll
+      for (int mi = 0; mi < 2; ++mi) {
+        mma16816(o[mi][2 * np], p[mi][kk], b0, b1);
+        mma16816(o[mi][2 * np + 1], p[mi][kk], b2, b3);
+      }
+    }
+  }
+}
+
+// Q | K | V tiles of 32 rows each, one after the other (temporal_attn_kernel's per-warp staging).
+struct TaTileRows {
+  const __half *Qs, *Ks, *Vs;
+  __device__ __forceinline__ const __half* q(int r) const { return Qs + r * TA_PITCH; }
+  __device__ __forceinline__ const __half* k(int r) const { return Ks + r * TA_PITCH; }
+  __device__ __forceinline__ const __half* v(int r) const { return Vs + r * TA_PITCH; }
+};
+
 __global__ void __launch_bounds__(TA_WARPS * 32) temporal_attn_kernel(const __half* __restrict__ q, const __half* __restrict__ k,
                                                                       const __half* __restrict__ v, int ld, __half* __restrict__ out,
                                                                       int ldo, int T, long long sites, int heads, float scale_log2) {
@@ -67,97 +173,8 @@ __global__ void __launch_bounds__(TA_WARPS * 32) temporal_attn_kernel(const __ha
     }
     __syncwarp();
 
-    // ---- S = Q K^T : [32 x 32], k = 64 ----
-    float s[2][4][4];
-#pragma unroll
-    for (int mi = 0; mi < 2; ++mi)
-#pragma unroll
-      for (int ni = 0; ni < 4; ++ni)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) s[mi][ni][e] = 0.f;
-    const int mat = lane >> 3, mr = lane & 7;
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      uint32_t a[2][4];
-#pragma unroll
-      for (int mi = 0; mi < 2; ++mi)
-        ldsm_x4(a[mi][0], a[mi][1], a[mi][2], a[mi][3], Qs + (mi * 16 + (mat & 1) * 8 + mr) * TA_PITCH + kk * 16 + (mat >> 1) * 8);
-#pragma unroll
-      for (int np = 0; np < 2; ++np) {                       // two n-tiles (16 keys) per ldmatrix.x4
-        uint32_t b0, b1, b2, b3;
-        ldsm_x4(b0, b1, b2, b3, Ks + (np * 16 + (mat >> 1) * 8 + mr) * TA_PITCH + kk * 16 + (mat & 1) * 8);
-#pragma unroll
-        for (int mi = 0; mi < 2; ++mi) {
-          mma16816(s[mi][2 * np], a[mi], b0, b1);
-          mma16816(s[mi][2 * np + 1], a[mi], b2, b3);
-        }
-      }
-    }
-
-    // ---- softmax over the key axis (columns); each thread owns rows g / g+8 of both m-tiles ----
-    uint32_t p[2][2][4];                                      // P as A fragments: [m-tile][k-step of 16 keys][4]
-    float inv_l[2][2];
-#pragma unroll
-    for (int mi = 0; mi < 2; ++mi) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {                           // h = 0: row g, h = 1: row g + 8
-        float mx = -INFINITY;
-#pragma unroll
-        for (int ni = 0; ni < 4; ++ni)
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int col = ni * 8 + 2 * tg + e;
-            float val = s[mi][ni][2 * h + e];
-            if (col >= T) val = -INFINITY;
-            s[mi][ni][2 * h + e] = val;
-            mx = fmaxf(mx, val);
-          }
-        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-        const float off = mx * scale_log2;
-        float l = 0.f;
-#pragma unroll
-        for (int ni = 0; ni < 4; ++ni)
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const float pv = exp2f(fmaf(s[mi][ni][2 * h + e], scale_log2, -off));
-            s[mi][ni][2 * h + e] = pv;
-            l += pv;
-          }
-        l += __shfl_xor_sync(0xffffffffu, l, 1);
-        l += __shfl_xor_sync(0xffffffffu, l, 2);
-        inv_l[mi][h] = 1.f / l;
-      }
-#pragma unroll
-      for (int kk = 0; kk < 2; ++kk) {
-        p[mi][kk][0] = pack_half2(s[mi][2 * kk][0], s[mi][2 * kk][1]);
-        p[mi][kk][1] = pack_half2(s[mi][2 * kk][2], s[mi][2 * kk][3]);
-        p[mi][kk][2] = pack_half2(s[mi][2 * kk + 1][0], s[mi][2 * kk + 1][1]);
-        p[mi][kk][3] = pack_half2(s[mi][2 * kk + 1][2], s[mi][2 * kk + 1][3]);
-      }
-    }
-
-    // ---- O = P V : [32 x 64], k = 32 keys ----
-    float o[2][8][4];
-#pragma unroll
-    for (int mi = 0; mi < 2; ++mi)
-#pragma unroll
-      for (int ni = 0; ni < 8; ++ni)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) o[mi][ni][e] = 0.f;
-#pragma unroll
-    for (int kk = 0; kk < 2; ++kk) {
-#pragma unroll
-      for (int np = 0; np < 4; ++np) {                       // two d-tiles (16 columns) per ldmatrix.x4.trans
-        uint32_t b0, b1, b2, b3;
-        ldsm_x4_t(b0, b1, b2, b3, Vs + (kk * 16 + (mat & 1) * 8 + mr) * TA_PITCH + np * 16 + (mat >> 1) * 8);
-#pragma unroll
-        for (int mi = 0; mi < 2; ++mi) {
-          mma16816(o[mi][2 * np], p[mi][kk], b0, b1);
-          mma16816(o[mi][2 * np + 1], p[mi][kk], b2, b3);
-        }
-      }
-    }
+    float o[2][8][4], inv_l[2][2];
+    ta_tile32(TaTileRows{Qs, Ks, Vs}, T, scale_log2, lane, o, inv_l);
 
     // ---- O / l -> smem (reuse the Q tile) -> coalesced 16-byte row stores ----
     __syncwarp();
@@ -405,6 +422,172 @@ int temporal_attn(const __half* q, const __half* k, const __half* v, int ld, __h
   if (blocks > cap) blocks = cap;
   temporal_attn_kernel<<<(unsigned)blocks, TA_WARPS * 32, TA_SMEM, stream>>>(q, k, v, ld, out, ldo, T, sites, heads,
                                                                             scale * 1.4426950408889634f);
+  VC_CHECK_CUDA(cudaGetLastError());
+  return VC_OK;
+}
+
+
+// ------------------------------------------------------------------------------------------------ windowed (FreeNoise)
+// Windowed temporal attention: overlapping windows of W <= 32 frames at starts 0, S, 2S, ... (while start + W < T) and T - W; frame
+// j of a window carries the weight min(j + 1, W - j) and out_t is the weighted mean of the outputs of the windows that contain t,
+// summed in window order (INTEGRATION.md "Long clips: windowed temporal attention").  T > W only (T <= W is the plain kernel).
+// One warp per (site, head) pair walks its windows in order; each window is ta_tile32 on shared-memory rows.  Frames stream
+// through a TW_RING-frame Q/K/V ring in chunks of 16 with cp.async, up to TW_RING - W frames ahead of the window, so each input row is
+// read from HBM once per pair.  The weighted fp32 sums of the open frames (at most W of them) live in a TW_ACC-row ring; a frame
+// is divided by its weight sum and written out once the next window starts past it.  Shared memory is O(W), independent of T.
+static constexpr int TW_WARPS = 2;
+static constexpr int TW_MAX_W = 32;
+static constexpr int TW_RING = 64;                                    // frames per Q/K/V ring (power of two, >= W + 16)
+static constexpr int TW_CHUNK = 16;                                   // frames per cp.async group
+static constexpr int TW_ACC = 32;                                     // open output rows (power of two, >= W)
+static constexpr int TW_ACC_PITCH = 72;                               // floats per accumulator row (conflict-free float2 access)
+static constexpr int TW_WARP_HALVES = 3 * TW_RING * TA_PITCH + TW_ACC * TW_ACC_PITCH * 2;
+static constexpr int TW_SMEM = (64 + TW_WARPS * TW_WARP_HALVES) * 2; // one zero row + per-warp rings
+static_assert(TW_ACC >= TW_MAX_W && TW_RING >= TW_MAX_W + TW_CHUNK, "ring sizes");
+
+// Window i of n (T > W): i * S, the last one T - W.  n = ceil((T - W) / S) + 1.
+__host__ __device__ __forceinline__ int tw_windows(int T, int W, int S) { return (T - W + S - 1) / S + 1; }
+__host__ __device__ __forceinline__ int tw_start(int i, int n, int T, int W, int S) { return i == n - 1 ? T - W : i * S; }
+// sum of min(j + 1, W - j) over the windows that contain frame t (j = t - start), from (t, T, W, S) alone
+__host__ __device__ __forceinline__ int tw_weight_sum(int t, int T, int W, int S) {
+  const int n = tw_windows(T, W, S);
+  int sum = 0;
+  for (int i = t < W ? 0 : (t - W) / S + 1; i < n - 1 && i * S <= t; ++i) {
+    const int j = t - i * S;
+    sum += min(j + 1, W - j);
+  }
+  if (t >= T - W) sum += min(t - (T - W) + 1, T - t);
+  return sum;
+}
+
+// Q | K | V rings; window rows r >= W read the shared zero row
+struct TwRingRows {
+  const __half* ring;
+  const __half* zero;
+  int start, W;
+  __device__ __forceinline__ const __half* row(int which, int r) const {
+    return r < W ? ring + (which * TW_RING + ((start + r) & (TW_RING - 1))) * TA_PITCH : zero;
+  }
+  __device__ __forceinline__ const __half* q(int r) const { return row(0, r); }
+  __device__ __forceinline__ const __half* k(int r) const { return row(1, r); }
+  __device__ __forceinline__ const __half* v(int r) const { return row(2, r); }
+};
+
+// frames 16c .. 16c + 15 of one pair into the rings (frames >= T are zero-filled), one cp.async group
+__device__ __forceinline__ void tw_load_chunk(__half* ring, const __half* __restrict__ q, const __half* __restrict__ k,
+                                              const __half* __restrict__ v, int ld, int T, long long sites, long long site, int head,
+                                              int c, int lane) {
+  const int lrow = lane >> 3, lchunk = (lane & 7) * 8;
+#pragma unroll
+  for (int j = 0; j < 3 * TW_CHUNK / 4; ++j) {
+    const int which = j / (TW_CHUNK / 4), t = c * TW_CHUNK + (j % (TW_CHUNK / 4)) * 4 + lrow;
+    const __half* src = which == 0 ? q : which == 1 ? k : v;
+    const bool valid = t < T;
+    const long long off = valid ? ((long long)t * sites + site) * ld + head * 64 + lchunk : 0;
+    cp_async16(ring + (which * TW_RING + (t & (TW_RING - 1))) * TA_PITCH + lchunk, src + off, valid);
+  }
+  cp_async_commit();
+}
+
+__global__ void __launch_bounds__(TW_WARPS * 32) temporal_attn_windowed_kernel(const __half* __restrict__ q, const __half* __restrict__ k,
+                                                                             const __half* __restrict__ v, int ld, __half* __restrict__ out,
+                                                                             int ldo, int T, long long sites, int heads, int W, int S,
+                                                                             float scale_log2) {
+  extern __shared__ __align__(16) __half tw_smem[];
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int g = lane >> 2, tg = lane & 3;
+  const int lrow = lane >> 3, lchunk = (lane & 7) * 8;
+  const __half* zero = tw_smem;
+  __half* ring = tw_smem + 64 + w * TW_WARP_HALVES;
+  float* acc = reinterpret_cast<float*>(ring + 3 * TW_RING * TA_PITCH);
+  if (threadIdx.x < 8) reinterpret_cast<uint4*>(tw_smem)[threadIdx.x] = make_uint4(0, 0, 0, 0);
+  for (int i = lane; i < TW_ACC * TW_ACC_PITCH / 4; i += 32) reinterpret_cast<float4*>(acc)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  __syncthreads();                                                    // the zero row is shared by the CTA's warps
+
+  const int nwin = tw_windows(T, W, S), nchunk = (T + TW_CHUNK - 1) / TW_CHUNK;
+  const long long pairs = sites * heads;
+  for (long long pair = (long long)blockIdx.x * TW_WARPS + w; pair < pairs; pair += (long long)gridDim.x * TW_WARPS) {
+    const long long site = pair / heads;
+    const int head = (int)(pair % heads);
+    int issued = 0;
+    for (int wi = 0; wi < nwin; ++wi) {
+      const int s0 = tw_start(wi, nwin, T, W, S);
+      const int s1 = wi + 1 < nwin ? tw_start(wi + 1, nwin, T, W, S) : T;   // frames [s0, s1) are complete after this window
+      // chunk c overwrites the ring rows of frames 16c - TW_RING ..: issue it once those are all below s0 (already consumed)
+      __syncwarp();
+      while (issued < nchunk && (issued + 1) * TW_CHUNK <= s0 + TW_RING) tw_load_chunk(ring, q, k, v, ld, T, sites, site, head, issued++, lane);
+      switch (issued - (s0 + W + TW_CHUNK - 1) / TW_CHUNK) {       // groups that may stay in flight: those past this window
+        case 0: cp_async_wait<0>(); break;
+        case 1: cp_async_wait<1>(); break;
+        case 2: cp_async_wait<2>(); break;
+        default: cp_async_wait<3>(); break;
+      }
+      __syncwarp();
+
+      float o[2][8][4], inv_l[2][2];
+      ta_tile32(TwRingRows{ring, zero, s0, W}, W, scale_log2, lane, o, inv_l);
+
+      // ---- acc[t] += w_j * O_j (fp32, window order) ----
+#pragma unroll
+      for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = mi * 16 + g + 8 * h;
+          if (r < W) {
+            const float wt = (float)min(r + 1, W - r);
+            float* a = acc + ((s0 + r) & (TW_ACC - 1)) * TW_ACC_PITCH + 2 * tg;
+#pragma unroll
+            for (int ni = 0; ni < 8; ++ni) {
+              float2 cur = *reinterpret_cast<float2*>(a + ni * 8);
+              cur.x += wt * (o[mi][ni][2 * h] * inv_l[mi][h]);
+              cur.y += wt * (o[mi][ni][2 * h + 1] * inv_l[mi][h]);
+              *reinterpret_cast<float2*>(a + ni * 8) = cur;
+            }
+          }
+        }
+      __syncwarp();
+
+      // ---- frames [s0, s1): / weight sum -> fp16 -> 16-byte row stores; their accumulator rows are cleared for reuse ----
+      for (int t = s0 + lrow; t < s1; t += 4) {
+        float4* a = reinterpret_cast<float4*>(acc + (t & (TW_ACC - 1)) * TW_ACC_PITCH + lchunk);
+        const float ws = (float)tw_weight_sum(t, T, W, S);
+        const float4 a0 = a[0], a1 = a[1];
+        uint4 r;
+        r.x = pack_half2(a0.x / ws, a0.y / ws);
+        r.y = pack_half2(a0.z / ws, a0.w / ws);
+        r.z = pack_half2(a1.x / ws, a1.y / ws);
+        r.w = pack_half2(a1.z / ws, a1.w / ws);
+        *reinterpret_cast<uint4*>(out + ((long long)t * sites + site) * ldo + head * 64 + lchunk) = r;
+        a[0] = a[1] = make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+    }
+  }
+  cp_async_wait<0>();
+}
+
+int temporal_attn_windowed(const __half* q, const __half* k, const __half* v, int ld, __half* out, int ldo, int T, long long sites,
+                           int heads, int W, int S, float scale, cudaStream_t stream) {
+  VC_REQUIRE(T >= 1, "temporal_attn_windowed: T=%d unsupported (>= 1)", T);
+  VC_REQUIRE(W >= 2 && W <= TW_MAX_W, "temporal_attn_windowed: window W=%d unsupported (2..%d)", W, TW_MAX_W);
+  VC_REQUIRE(S >= 1 && S <= W, "temporal_attn_windowed: stride S=%d unsupported (1..W=%d)", S, W);
+  VC_REQUIRE(q && k && v && out, "temporal_attn_windowed: null pointer");
+  VC_REQUIRE(ld % 8 == 0 && ldo % 8 == 0, "temporal_attn_windowed: pitches must be multiples of 8");
+  VC_REQUIRE(sites >= 1 && heads >= 1, "temporal_attn_windowed: sites=%lld heads=%d", sites, heads);
+  if (T <= W) return temporal_attn(q, k, v, ld, out, ldo, T, sites, heads, scale, stream);   // one window: full attention
+  static DeviceOnce configured;
+  if (device_once_needed(configured)) {
+    VC_CHECK_CUDA(cudaFuncSetAttribute(temporal_attn_windowed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TW_SMEM));
+    device_once_mark(configured);
+  }
+  int per_sm = 0;
+  VC_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, temporal_attn_windowed_kernel, TW_WARPS * 32, TW_SMEM));
+  VC_REQUIRE(per_sm >= 1, "temporal_attn_windowed: the kernel does not fit on an SM");
+  const long long pairs = sites * heads;
+  long long blocks = (pairs + TW_WARPS - 1) / TW_WARPS;
+  const long long cap = (long long)per_sm * sm_count();               // grid-stride beyond one resident wave
+  if (blocks > cap) blocks = cap;
+  temporal_attn_windowed_kernel<<<(unsigned)blocks, TW_WARPS * 32, TW_SMEM, stream>>>(q, k, v, ld, out, ldo, T, sites, heads, W, S,
+                                                                                      scale * 1.4426950408889634f);
   VC_CHECK_CUDA(cudaGetLastError());
   return VC_OK;
 }

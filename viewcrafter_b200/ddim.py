@@ -12,7 +12,7 @@ from __future__ import annotations
 import numpy as np
 import torch
 
-from . import ops, schedule
+from . import ops, schedule, temporal_window
 
 
 def check_row_replay(opts: dict):
@@ -128,13 +128,18 @@ class DDIMSampler(object):
                       quantize_denoised=False, mask=None, x0=None, img_callback=None, log_every_t=100, temperature=1.,
                       noise_dropout=0., score_corrector=None, corrector_kwargs=None, unconditional_guidance_scale=1.,
                       unconditional_conditioning=None, verbose=True, precision=None, fs=None, guidance_rescale=0.0, _rng_rows=None,
-                      **kwargs):
+                      window_seed=0, **kwargs):
+        """window_seed: while the U-Net has a temporal window set (UNetModel.set_temporal_window), a drawn x_T is rescheduled with
+        temporal_window.reschedule_noise(seed=window_seed) after the draw; an explicit x_T is used as given."""
         if ddim_use_original_steps:
             # the reference's own branch reads self.ddim_sigmas_for_original_num_steps, which its make_schedule never defines (ddim.py:248)
             raise NotImplementedError("viewcrafter_b200.DDIMSampler: ddim_use_original_steps is not implemented (it fails in the reference too)")
         device = self._device()
         b = shape[0]
         img = torch.randn(shape, device=device) if x_T is None else x_T
+        window = getattr(getattr(getattr(self.model, "model", None), "diffusion_model", None), "temporal_window", None)
+        if x_T is None and window is not None:            # every batch row alike, so _rng_rows keeps row b of the rescheduled batch
+            img = temporal_window.reschedule_noise(img, window, window_seed)
         rng_batch = None
         if _rng_rows is not None:                           # sample(_rng_rows=...): keep rows b0:b1 of the batch's draws (_step_noise too)
             img, b = img[_rng_rows[0]:_rng_rows[1]].contiguous(), _rng_rows[1] - _rng_rows[0]

@@ -477,6 +477,20 @@ def temporal_attn(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, T: int, sit
     return out
 
 
+def temporal_attn_windowed(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, T: int, sites: int, heads: int, W: int, S: int,
+                           scale: float = 0.125, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """temporal_attn on overlapping windows of W frames with stride S, blended per frame with the weights min(j + 1, W - j)
+    (vc_temporal_attn_windowed; INTEGRATION.md "Long clips: windowed temporal attention").  T <= W is temporal_attn exactly."""
+    _chk16(q, "tattn_win.q")
+    if out is None:
+        out = torch.empty((T * sites, heads * 64), device=q.device, dtype=torch.float16)
+    assert out.shape == (T * sites, heads * 64) and out.dtype == torch.float16 and out.stride(1) == 1
+    assert q.stride(0) == k.stride(0) == v.stride(0)
+    check(_lib.load().vc_temporal_attn_windowed(q.data_ptr(), k.data_ptr(), v.data_ptr(), q.stride(0), out.data_ptr(), out.stride(0),
+                                                T, sites, heads, W, S, scale, _stream()), "vc_temporal_attn_windowed")
+    return out
+
+
 # ----------------------------------------------------------------------------------------------------
 # normalisation / data movement
 # ----------------------------------------------------------------------------------------------------

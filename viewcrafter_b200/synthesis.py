@@ -21,9 +21,11 @@ What differs from the reference, all parity-preserving (SURVEY.md App. C):
 """
 from __future__ import annotations
 
+import contextlib
+
 import torch
 
-from . import ops, parallel
+from . import ops, parallel, temporal_window as _tw
 from .ddim import DDIMSampler, check_row_replay
 from .ddim_multiplecond import DDIMSampler as DDIMSampler_multicond
 from .dpm_solver import DPMSolver3MSDESampler, DPMSolver3MSDESamplerMultiCond, DPMSolverSampler, DPMSolverSamplerMultiCond
@@ -53,27 +55,48 @@ def get_latent_z(model, videos):
 def image_guided_synthesis(model, prompts, videos, noise_shape, n_samples=1, ddim_steps=50, ddim_eta=1.,
                            unconditional_guidance_scale=1.0, cfg_img=None, fs=None, text_input=False, multiple_cond_cfg=False,
                            timestep_spacing='uniform', guidance_rescale=0.0, condition_index=None, batch_cfg=True, cuda_graph=True,
-                           reproducible=None, sampler="ddim", **kwargs):
+                           reproducible=None, sampler="ddim", temporal_window=None, window_seed=0, **kwargs):
     """reproducible: True / False switches viewcrafter_b200's reproducible mode (ops.set_reproducible) for this call and restores the
     previous setting afterwards; None leaves the process setting as it is.
     sampler: "ddim" (the reference's DDIMSampler), "dpmpp_2m" (dpm_solver.DPMSolverSampler / DPMSolverSamplerMultiCond, which takes
     ddim_eta 0 or 1 only) or "dpmpp_3m_sde" (dpm_solver.DPMSolver3MSDESampler / DPMSolver3MSDESamplerMultiCond, ddim_eta 1 only;
-    INTEGRATION.md "Samplers")."""
+    INTEGRATION.md "Samplers").
+    temporal_window: None (full temporal attention) or (W, S): the U-Net runs windowed temporal attention for this call and the drawn
+    x_T is rescheduled with window_seed (FreeNoise; INTEGRATION.md "Long clips: windowed temporal attention").  The U-Net's previous
+    setting is restored afterwards.  An explicit x_T= is used as given, without rescheduling."""
     if sampler not in SAMPLERS:
         raise ValueError(f"unknown sampler {sampler!r}; choose one of {sorted(SAMPLERS)}")
     if sampler != "ddim":
         SAMPLERS[sampler][0].check_eta(ddim_eta)          # before the conditioning is computed
-    if reproducible is None:
-        return _synthesis(model, prompts, videos, noise_shape, n_samples, ddim_steps, ddim_eta, unconditional_guidance_scale, cfg_img, fs,
-                          text_input, multiple_cond_cfg, timestep_spacing, guidance_rescale, condition_index, batch_cfg, cuda_graph,
-                          sampler=sampler, **kwargs)
-    prev = ops.set_reproducible(reproducible)
+    with _unet_window(model, _tw.check_window(temporal_window)):
+        if reproducible is None:
+            return _synthesis(model, prompts, videos, noise_shape, n_samples, ddim_steps, ddim_eta, unconditional_guidance_scale, cfg_img,
+                              fs, text_input, multiple_cond_cfg, timestep_spacing, guidance_rescale, condition_index, batch_cfg, cuda_graph,
+                              sampler=sampler, window_seed=window_seed, **kwargs)
+        prev = ops.set_reproducible(reproducible)
+        try:
+            return _synthesis(model, prompts, videos, noise_shape, n_samples, ddim_steps, ddim_eta, unconditional_guidance_scale, cfg_img,
+                              fs, text_input, multiple_cond_cfg, timestep_spacing, guidance_rescale, condition_index, batch_cfg, cuda_graph,
+                              sampler=sampler, window_seed=window_seed, **kwargs)
+        finally:
+            ops.set_reproducible(prev)
+
+
+@contextlib.contextmanager
+def _unet_window(model, window):
+    """The U-Net's temporal window set to `window` (None: off) inside the block and restored after it."""
+    unet = getattr(getattr(model, "model", None), "diffusion_model", None)
+    if not hasattr(unet, "set_temporal_window"):
+        if window is not None:
+            raise ValueError("image_guided_synthesis: temporal_window needs the viewcrafter_b200 UNetModel")
+        yield
+        return
+    prev = unet.temporal_window
+    unet.set_temporal_window(window)
     try:
-        return _synthesis(model, prompts, videos, noise_shape, n_samples, ddim_steps, ddim_eta, unconditional_guidance_scale, cfg_img, fs,
-                          text_input, multiple_cond_cfg, timestep_spacing, guidance_rescale, condition_index, batch_cfg, cuda_graph,
-                          sampler=sampler, **kwargs)
+        yield
     finally:
-        ops.set_reproducible(prev)
+        unet.set_temporal_window(prev)
 
 
 def _synthesis(model, prompts, videos, noise_shape, n_samples, ddim_steps, ddim_eta, unconditional_guidance_scale, cfg_img, fs, text_input,

@@ -21,7 +21,7 @@ from typing import List, Optional
 import torch
 import torch.nn as nn
 
-from . import ops
+from . import ops, temporal_window
 
 
 def _zero(m: nn.Module) -> nn.Module:
@@ -274,6 +274,7 @@ class UNetModel(nn.Module):
         self._graphs = {}
         self.graph_replayed_launches = 0    # kernels of this library executed through graph replays (bench.py's gpu_launches)
         self._fp8, self._packed8 = False, None
+        self._twin = None           # temporal attention window (W, S), see set_temporal_window
         self.register_load_state_dict_post_hook(lambda module, incompatible: module.invalidate_packed())
 
     # ------------------------------------------------------------------------------------------
@@ -319,6 +320,20 @@ class UNetModel(nn.Module):
 
     def fp8_enabled(self) -> bool:
         return self._fp8
+
+    def set_temporal_window(self, window=None):
+        """Windowed temporal attention (FreeNoise; INTEGRATION.md "Long clips: windowed temporal attention"): with window = (W, S),
+        2 <= W <= 32, 1 <= S <= W, every temporal self-attention (attn1 and attn2 of every TemporalTransformer, and init_attn) of a
+        clip of T > W frames runs on overlapping windows of W frames with stride S, blended per frame.  Temporal convolutions,
+        GroupNorms, spatial and cross-attention are unchanged.  None (the default) is full temporal attention.  The samplers
+        reschedule a drawn x_T while a window is set (temporal_window.reschedule_noise).  Raises ValueError out of range."""
+        self._twin = temporal_window.check_window(window)
+        return self
+
+    @property
+    def temporal_window(self):
+        """The (W, S) set by set_temporal_window, or None."""
+        return self._twin
 
     def _packs(self):
         """The packed operands of the current mode (fp16, or the FP8 packs built from them)."""
@@ -507,8 +522,10 @@ class UNetModel(nn.Module):
         return ops.linear(x, P["out_w"], bias=P["out_b"], res=h, gn_out=True, peer=out_plan)
 
     @staticmethod
-    def _temporal_tf(P, h, B, T, H, W, comm=None, pre_sites=False):
-        """pre_sites: `h` already is in the site layout (the producing GEMM switched it, see _spatial_tf(out_plan=...))."""
+    def _temporal_tf(P, h, B, T, H, W, comm=None, pre_sites=False, window=None):
+        """pre_sites: `h` already is in the site layout (the producing GEMM switched it, see _spatial_tf(out_plan=...)).
+        window: (W, S) of set_temporal_window or None.  Under frame sharding each rank holds all frames of its sites, so the
+        windows are local too."""
         HW, heads = H * W, P["heads"]
         C = heads * 64
         Tg, HWl = (comm.T, HW // comm.world) if comm else (T, HW)
@@ -521,7 +538,11 @@ class UNetModel(nn.Module):
                 a = torch.empty((qkv.shape[0], C), device=qkv.device, dtype=torch.float16)
                 for b in range(B):
                     rows = slice(b * Tg * HWl, (b + 1) * Tg * HWl)
-                    ops.temporal_attn(qkv[rows, :C], qkv[rows, C:2 * C], qkv[rows, 2 * C:], Tg, HWl, heads, out=a[rows])
+                    if window is not None and Tg > window[0]:
+                        ops.temporal_attn_windowed(qkv[rows, :C], qkv[rows, C:2 * C], qkv[rows, 2 * C:], Tg, HWl, heads, *window,
+                                                   out=a[rows])
+                    else:
+                        ops.temporal_attn(qkv[rows, :C], qkv[rows, C:2 * C], qkv[rows, 2 * C:], Tg, HWl, heads, out=a[rows])
                 x, st = ops.linear(a, Q[ow], bias=Q[ob], res=x, ln_out=True)
             x, st = _ff(Q, x, st, Q is P["blocks"][-1])
         to_f = comm.scatter_plan(False, B, HW, P["out_w"].shape[0]) if comm else None
@@ -541,7 +562,7 @@ class UNetModel(nn.Module):
                 h = self._spatial_tf(P, h, ctx, B, T, H, W, out_plan=plan)
                 pre_sites = plan is not None
             elif k == "T":
-                h = self._temporal_tf(P, h, B, T, H, W, comm, pre_sites=pre_sites)
+                h = self._temporal_tf(P, h, B, T, H, W, comm, pre_sites=pre_sites, window=self._twin)
                 pre_sites = False
             elif k == "D":
                 cols, H, W = ops.im2col_s2(h, B * T, H, W)
@@ -619,7 +640,7 @@ class UNetModel(nn.Module):
     def _forward_graphed(self, x, timesteps, context, fs, kwargs):
         ver = ops.tensor_version(context)
         flags = tuple(sorted((k, bool(v)) for k, v in kwargs.items() if k == "cfg_shared_prefix"))
-        key = (tuple(x.shape), x.dtype, id(context), ver, fs is None, flags, id(self._comm), self._fp8, ops.reproducible())
+        key = (tuple(x.shape), x.dtype, id(context), ver, fs is None, flags, id(self._comm), self._twin, self._fp8, ops.reproducible())
         e = self._graphs.get(key)
         if ver is None or (e is not None and e["ctx"] is not context):
             return self._forward_impl(x, timesteps, context, fs, kwargs)
