@@ -215,6 +215,22 @@ int vc_ddim_update(const float* x, const float* v_cond, const float* v_uncond, c
  * replaces: lvdm/models/samplers/ddim_multiplecond.py:227-236 (+ the shared tail :238-287) */
 int vc_ddim_update3(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img,
                     const float* noise, float* x_prev, float* pred_x0, int64_t n, const vc_ddim_scalars* s, void* ws /* 4 * 1025 doubles */, void* stream);
+/* DDIM update with a step per frame (FIFO-Diffusion's diagonal denoising, INTEGRATION.md "Long clips: FIFO diagonal denoising"): the
+ * inputs are laid out [B', C, T, HW] and element e belongs to frame (e / HW) % T, which takes frames[frame]'s scalars.  cfg_scale,
+ * guidance_rescale, use_cfg and reproducible come from `s` (its per-step fields are not read); two-way, or three-way when
+ * v_uncond_img is not null.  The guidance-rescale statistics run over all n elements, as in vc_ddim_update.  `frames` is a HOST
+ * array of T <= VC_DDIM_MAX_FRAMES entries, passed to the kernel by value, so the call can be captured in a CUDA graph.  With every
+ * frame's scalars equal to s's, x_prev and pred_x0 are vc_ddim_update's / vc_ddim_update3's bit for bit.
+ * New functionality (the reference has no per-frame timesteps). */
+#define VC_DDIM_MAX_FRAMES 128
+typedef struct vc_ddim_frame_scalars {
+  float sqrt_ac_t, sqrt_1mac_t;
+  float a_prev, sigma_t;
+  float scale_t, prev_scale_t;
+} vc_ddim_frame_scalars;
+int vc_ddim_update_frames(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img,
+                          const float* noise, float* x_prev, float* pred_x0, int64_t n, int32_t T, int64_t HW, const vc_ddim_scalars* s,
+                          const vc_ddim_frame_scalars* frames, void* ws /* 4 * 1025 doubles */, void* stream);
 /* DPM-Solver++(2M) step (INTEGRATION.md "Samplers"): the DDIM update above (two-way, or three-way when v_uncond_img is not null),
  * x_ddim, then x_prev = x_ddim + c_hist (x0 - x0_hist) with x0 = sqrt_ac_t x - sqrt_1mac_t v before the dynamic rescale; x0_hist
  * (n floats, read only when c_hist != 0) is overwritten with this step's x0.  c_hist = 0 gives vc_ddim_update's x_prev bit for bit.

@@ -11,6 +11,8 @@ Added samplers (opt-in; DDIM stays the default):
     viewcrafter_b200.dpm_solver.DPMSolverSampler / DPMSolverSamplerMultiCond: DPM-Solver++(2M), image_guided_synthesis(sampler="dpmpp_2m")
     viewcrafter_b200.dpm_solver.DPMSolver3MSDESampler / DPMSolver3MSDESamplerMultiCond: DPM-Solver++(3M) SDE (eta = 1),
         image_guided_synthesis(sampler="dpmpp_3m_sde")
+    viewcrafter_b200.fifo.FIFOSampler / FIFOSamplerMultiCond: FIFO-Diffusion diagonal denoising, clips of any length at the memory
+        of one window, image_guided_synthesis(fifo=f)
 All tensor work runs in libvc_b200.so (hand-written CUDA for sm_90a, C ABI in include/vc_b200.h).
 
 set_reproducible(on) / VC_REPRODUCIBLE=1: reproducible mode (bit-identical results across batching, GPU count and SM count).

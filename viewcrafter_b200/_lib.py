@@ -52,6 +52,14 @@ class DdimScalars(C.Structure):
                 ("scale_t", C.c_float), ("prev_scale_t", C.c_float), ("use_cfg", C.c_int32), ("reproducible", C.c_int32)]
 
 
+DDIM_MAX_FRAMES = 128      # VC_DDIM_MAX_FRAMES
+
+
+class DdimFrameScalars(C.Structure):
+    _fields_ = [("sqrt_ac_t", C.c_float), ("sqrt_1mac_t", C.c_float), ("a_prev", C.c_float), ("sigma_t", C.c_float),
+                ("scale_t", C.c_float), ("prev_scale_t", C.c_float)]
+
+
 class PeerComm(C.Structure):
     _fields_ = [("world", C.c_int32), ("rank", C.c_int32), ("flags", C.c_void_p), ("peer_flags", C.c_void_p * 8),
                 ("seq", C.c_void_p), ("done", C.c_void_p), ("stats_slots", C.c_void_p * 8), ("cur_stats", C.c_void_p),
@@ -108,6 +116,8 @@ SIGNATURES = {
     "vc_small_linear_f32": (C.c_int, [_vp, _i32, _i32, _vp, _vp, _i32, _i32, _vp, _vp, _vp]),
     "vc_ddim_update": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, C.POINTER(DdimScalars), _vp, _vp]),
     "vc_ddim_update3": (C.c_int, [_vp, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _i64, C.POINTER(DdimScalars), _vp, _vp]),
+    "vc_ddim_update_frames": (C.c_int, [_vp, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _i64, _i32, _i64, C.POINTER(DdimScalars),
+                                        C.POINTER(DdimFrameScalars), _vp, _vp]),
     "vc_dpm_update": (C.c_int, [_vp, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _vp, _i64, C.POINTER(DdimScalars), _f32, _vp, _vp]),
     "vc_dpm3_update": (C.c_int, [_vp, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _vp, _vp, _i64, C.POINTER(DdimScalars), _f32, _f32, _vp, _vp]),
 }

@@ -176,6 +176,15 @@ int vc_ddim_update3(const float* x, const float* v_cond, const float* v_uncond, 
   COUNT((s->use_cfg && s->guidance_rescale > 0.f) ? 2 : 1);
   return ddim_update(x, v_cond, v_uncond, v_uncond_img, cfg_img, noise, x_prev, pred_x0, n, *s, reinterpret_cast<double*>(ws), ST(stream));
 }
+int vc_ddim_update_frames(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img,
+                          const float* noise, float* x_prev, float* pred_x0, int64_t n, int32_t T, int64_t HW, const vc_ddim_scalars* s,
+                          const vc_ddim_frame_scalars* frames, void* ws, void* stream) {
+  if (!s) { set_error("vc_ddim_update_frames: null scalars"); return VC_ERR_ARG; }
+  const int rc = ddim_update_frames(x, v_cond, v_uncond, v_uncond_img, cfg_img, noise, x_prev, pred_x0, n, T, HW, *s, frames,
+                                    reinterpret_cast<double*>(ws), ST(stream));
+  if (rc == VC_OK) COUNT((s->use_cfg && s->guidance_rescale > 0.f) ? 2 : 1);
+  return rc;
+}
 int vc_dpm_update(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img,
                   const float* noise, float* x0_hist, float* x_prev, float* pred_x0, int64_t n, const vc_ddim_scalars* s, float c_hist,
                   void* ws, void* stream) {

@@ -74,6 +74,10 @@ int timestep_embedding_f32(const long long* t, int n, int dim, float* out, cudaS
 // v_uncond_img != nullptr: three-way CFG of ddim_multiplecond.py:227-233 with weight cfg_img on the image-only branch
 int ddim_update(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img, const float* noise,
                 float* x_prev, float* pred_x0, long long n, const vc_ddim_scalars& s, double* ws, cudaStream_t stream);
+// ddim_update with a step per frame: element i of [B', C, T, HW] takes frames[(i / HW) % T] (host array, T <= VC_DDIM_MAX_FRAMES)
+int ddim_update_frames(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img,
+                       const float* noise, float* x_prev, float* pred_x0, long long n, int T, long long HW, const vc_ddim_scalars& s,
+                       const vc_ddim_frame_scalars* frames, double* ws, cudaStream_t stream);
 // ddim_update plus the DPM-Solver++(2M) correction x_prev += c_hist (x0 - x0_hist); x0_hist <- this step's x0 (before the dynamic rescale)
 int dpm_update(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img, const float* noise,
                float* x0_hist, float* x_prev, float* pred_x0, long long n, const vc_ddim_scalars& s, float c_hist, double* ws,

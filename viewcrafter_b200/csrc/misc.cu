@@ -1,6 +1,8 @@
 // Small / HBM-bound kernels of the denoise step:
 // nearest-2x upsample, stride-2 im2col, layout conversions, the timestep/fps embedding MLP pieces
 // and the fused DDIM update.
+#include <cstring>
+
 #include "common.cuh"
 #include "kernels.h"
 
@@ -295,60 +297,137 @@ __global__ void __launch_bounds__(256) ddim_stats_kernel(const float* __restrict
     ws[4 + 4 * blockIdx.x + threadIdx.x] = a;
   }
 }
+// The pieces of the DDIM apply step, shared by ddim_apply_kernel (one step for the whole input) and ddim_frames_apply_kernel (a step
+// per frame), so both evaluate the same expressions in the same order.
+// guidance-rescale factor std(v_cond) / std(guided v) from the statistics blocks' partial sums, added up in index order
+__device__ __forceinline__ float ddim_rescale_factor(const double* ws, int stat_blocks, long long n) {
+  __shared__ double tot[4];
+  if (threadIdx.x < 4) {
+    double a = 0;
+    for (int b = 0; b < stat_blocks; ++b) a += ws[4 + 4 * b + threadIdx.x];
+    tot[threadIdx.x] = a;
+  }
+  __syncthreads();
+  const double dn = (double)n;
+  const double var_t = (tot[1] - tot[0] * tot[0] / dn) / (dn - 1.0);
+  const double var_c = (tot[3] - tot[2] * tot[2] / dn) / (dn - 1.0);
+  return (float)sqrt(var_t > 0 ? var_t : 0.0) / (float)sqrt(var_c > 0 ? var_c : 0.0);
+}
+// the step's scalars and the constants derived from them
+struct DdimStep {
+  float sqrt_ac_t, sqrt_1mac_t, sigma_t, rescale, dir_c, sq_ap;
+};
+__device__ __forceinline__ DdimStep ddim_step(float sqrt_ac_t, float sqrt_1mac_t, float a_prev, float sigma_t, float scale_t,
+                                              float prev_scale_t) {
+  DdimStep d;
+  d.sqrt_ac_t = sqrt_ac_t; d.sqrt_1mac_t = sqrt_1mac_t; d.sigma_t = sigma_t;
+  d.rescale = __fdiv_rn(prev_scale_t, scale_t);
+  // eta = 1 from a = 0: 1 - a' - sigma^2 is 0 in exact arithmetic, and the contracted FADD + FFMA of the fp32 step scalars lands
+  // below 0 at many step counts (uniform_trailing S = 4, 7, 9, 25, ...), where an unclamped sqrtf turns every x_prev into NaN.
+  // Clamped; the same bits wherever it is >= 0, and the same expression as dpm_apply_kernel (c_hist = 0 is this update bit for bit)
+  d.dir_c = sqrtf(fmaxf(__fmaf_rn(-sigma_t, sigma_t, __fsub_rn(1.f, a_prev)), 0.f));
+  d.sq_ap = sqrtf(a_prev);
+  return d;
+}
+// element i: guided v, then pred_x0 and x_prev.  Every rounding is spelled out (the _rn intrinsics are never contracted), in the
+// order and with the fused products ptxas chose for the contracted expressions of the original single-step kernel
+// (u + s (c - u), (u + s_img (vi - u)) + s (c - vi), g (m factor) + (1 - g) m, sqrt_ac m + sqrt_1mac x, sqrt_ac x - sqrt_1mac m,
+// sq_ap p0 + dir_c e_t + sigma noise): its outputs are unchanged, and a kernel that runs this code with the same step gets its bits
+// whatever ptxas does around it.
+__device__ __forceinline__ void ddim_element(const float* __restrict__ x, const float* __restrict__ vc_, const float* __restrict__ vu,
+                                             const float* __restrict__ vi, float cfg_img, const float* __restrict__ noise,
+                                             float* __restrict__ x_prev, float* __restrict__ pred_x0, long long i,
+                                             const vc_ddim_scalars& s, float factor, const DdimStep& d) {
+  const float c = vc_[i];
+  float m = c;
+  if (s.use_cfg) {
+    const float u = vu[i];
+    if (vi == nullptr) {
+      m = __fmaf_rn(__fsub_rn(c, u), s.cfg_scale, u);
+    } else {
+      const float w = vi[i];
+      m = __fmaf_rn(__fsub_rn(c, w), s.cfg_scale, __fmaf_rn(__fsub_rn(w, u), cfg_img, u));
+    }
+    if (s.guidance_rescale > 0.f)
+      m = __fmaf_rn(m, __fsub_rn(1.f, s.guidance_rescale), __fmul_rn(__fmul_rn(m, factor), s.guidance_rescale));
+  }
+  const float xi = x[i];
+  const float e_t = __fmaf_rn(m, d.sqrt_ac_t, __fmul_rn(xi, d.sqrt_1mac_t));
+  float p0 = __fmaf_rn(xi, d.sqrt_ac_t, -__fmul_rn(m, d.sqrt_1mac_t));
+  p0 = __fmul_rn(p0, d.rescale);
+  pred_x0[i] = p0;
+  x_prev[i] = __fmaf_rn(noise[i], d.sigma_t, __fmaf_rn(e_t, d.dir_c, __fmul_rn(p0, d.sq_ap)));
+}
 __global__ void ddim_apply_kernel(const float* __restrict__ x, const float* __restrict__ vc_, const float* __restrict__ vu,
                                   const float* __restrict__ vi, float cfg_img,
                                   const float* __restrict__ noise, float* __restrict__ x_prev, float* __restrict__ pred_x0,
                                   long long n, vc_ddim_scalars s, const double* ws, int stat_blocks) {
   float factor = 1.f;
-  if (s.use_cfg && s.guidance_rescale > 0.f) {
-    __shared__ double tot[4];
-    if (threadIdx.x < 4) {
-      double a = 0;
-      for (int b = 0; b < stat_blocks; ++b) a += ws[4 + 4 * b + threadIdx.x];
-      tot[threadIdx.x] = a;
-    }
-    __syncthreads();
-    const double dn = (double)n;
-    const double var_t = (tot[1] - tot[0] * tot[0] / dn) / (dn - 1.0);
-    const double var_c = (tot[3] - tot[2] * tot[2] / dn) / (dn - 1.0);
-    factor = (float)sqrt(var_t > 0 ? var_t : 0.0) / (float)sqrt(var_c > 0 ? var_c : 0.0);
+  if (s.use_cfg && s.guidance_rescale > 0.f) factor = ddim_rescale_factor(ws, stat_blocks, n);
+  const DdimStep d = ddim_step(s.sqrt_ac_t, s.sqrt_1mac_t, s.a_prev, s.sigma_t, s.scale_t, s.prev_scale_t);
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    ddim_element(x, vc_, vu, vi, cfg_img, noise, x_prev, pred_x0, i, s, factor, d);
+}
+// per-frame step scalars, passed by value (kernel parameters: no host-to-device copy, so the launch can be captured in a CUDA graph)
+struct DdimFrameTable {
+  vc_ddim_frame_scalars f[VC_DDIM_MAX_FRAMES];
+};
+// element i of [B', C, T, HW] belongs to frame (i / HW) % T and takes that frame's step; each CTA derives the T steps once
+__global__ void __launch_bounds__(256) ddim_frames_apply_kernel(const float* __restrict__ x, const float* __restrict__ vc_,
+                                  const float* __restrict__ vu, const float* __restrict__ vi, float cfg_img,
+                                  const float* __restrict__ noise, float* __restrict__ x_prev, float* __restrict__ pred_x0,
+                                  long long n, int T, long long HW, vc_ddim_scalars s, const __grid_constant__ DdimFrameTable tab,
+                                  const double* ws, int stat_blocks) {
+  __shared__ DdimStep steps[VC_DDIM_MAX_FRAMES];
+  for (int f = threadIdx.x; f < T; f += blockDim.x) {
+    const vc_ddim_frame_scalars& q = tab.f[f];
+    steps[f] = ddim_step(q.sqrt_ac_t, q.sqrt_1mac_t, q.a_prev, q.sigma_t, q.scale_t, q.prev_scale_t);
   }
-  const float rescale = s.prev_scale_t / s.scale_t;
-  // eta = 1 from a = 0: 1 - a' - sigma^2 is 0 in exact arithmetic, and the contracted FADD + FFMA of the fp32 step scalars lands
-  // below 0 at many step counts (uniform_trailing S = 4, 7, 9, 25, ...), where an unclamped sqrtf turns every x_prev into NaN.
-  // Clamped; the same bits wherever it is >= 0, and the same expression as dpm_apply_kernel (c_hist = 0 is this update bit for bit)
-  const float dir_c = sqrtf(fmaxf(1.f - s.a_prev - s.sigma_t * s.sigma_t, 0.f));
-  const float sq_ap = sqrtf(s.a_prev);
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    const float c = vc_[i];
-    float m = c;
-    if (s.use_cfg) {
-      const float u = vu[i];
-      m = cfg_combine(c, u, vi, i, s.cfg_scale, cfg_img);
-      if (s.guidance_rescale > 0.f) m = s.guidance_rescale * (m * factor) + (1.f - s.guidance_rescale) * m;
-    }
-    const float xi = x[i];
-    const float e_t = s.sqrt_ac_t * m + s.sqrt_1mac_t * xi;
-    float p0 = s.sqrt_ac_t * xi - s.sqrt_1mac_t * m;
-    p0 *= rescale;
-    pred_x0[i] = p0;
-    x_prev[i] = sq_ap * p0 + dir_c * e_t + s.sigma_t * noise[i];
-  }
+  float factor = 1.f;
+  if (s.use_cfg && s.guidance_rescale > 0.f) factor = ddim_rescale_factor(ws, stat_blocks, n);
+  __syncthreads();
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    ddim_element(x, vc_, vu, vi, cfg_img, noise, x_prev, pred_x0, i, s, factor, steps[(int)((i / HW) % T)]);
+}
+// the grid of the statistics and apply kernels.  Reproducible mode: a fixed number of statistics blocks, so the grid-strided order
+// of the two std reductions does not depend on the SM count
+static int ddim_blocks(long long n, const vc_ddim_scalars& s) {
+  int blocks = (int)min(s.reproducible ? (long long)DDIM_REPRO_BLOCKS : (long long)sm_count() * 4, (n + 255) / 256);
+  return blocks > DDIM_MAX_BLOCKS ? DDIM_MAX_BLOCKS : blocks;
 }
 int ddim_update(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img, const float* noise,
                 float* x_prev, float* pred_x0, long long n, const vc_ddim_scalars& s, double* ws, cudaStream_t stream) {
   VC_REQUIRE(x && v_cond && noise && x_prev && pred_x0 && ws && n > 1, "ddim_update: bad args");
   VC_REQUIRE(!s.use_cfg || v_uncond, "ddim_update: CFG needs the unconditional output");
   VC_REQUIRE(!v_uncond_img || s.use_cfg, "ddim_update: the image-only branch is only defined with CFG on");
-  // reproducible mode: a fixed number of statistics blocks, so the grid-strided order of the two std reductions does not depend on
-  // the SM count
-  int blocks = (int)min(s.reproducible ? (long long)DDIM_REPRO_BLOCKS : (long long)sm_count() * 4, (n + 255) / 256);
-  if (blocks > DDIM_MAX_BLOCKS) blocks = DDIM_MAX_BLOCKS;
+  const int blocks = ddim_blocks(n, s);
   if (s.use_cfg && s.guidance_rescale > 0.f) {           // ws: 4 * (1 + DDIM_MAX_BLOCKS) doubles
     ddim_stats_kernel<<<blocks, 256, 0, stream>>>(v_cond, v_uncond, v_uncond_img, n, s.cfg_scale, cfg_img, ws);
     VC_CHECK_CUDA(cudaGetLastError());
   }
   ddim_apply_kernel<<<blocks, 256, 0, stream>>>(x, v_cond, v_uncond, v_uncond_img, cfg_img, noise, x_prev, pred_x0, n, s, ws, blocks);
+  VC_CHECK_CUDA(cudaGetLastError());
+  return VC_OK;
+}
+int ddim_update_frames(const float* x, const float* v_cond, const float* v_uncond, const float* v_uncond_img, float cfg_img,
+                       const float* noise, float* x_prev, float* pred_x0, long long n, int T, long long HW, const vc_ddim_scalars& s,
+                       const vc_ddim_frame_scalars* frames, double* ws, cudaStream_t stream) {
+  VC_REQUIRE(x && v_cond && noise && x_prev && pred_x0 && ws && frames, "ddim_update_frames: null pointer");
+  VC_REQUIRE(T >= 1 && T <= VC_DDIM_MAX_FRAMES, "ddim_update_frames: T=%d unsupported (1..%d)", T, VC_DDIM_MAX_FRAMES);
+  VC_REQUIRE(HW >= 1 && n > 1 && n % ((long long)T * HW) == 0, "ddim_update_frames: n=%lld is not a multiple of T*HW=%lld", n,
+             (long long)T * HW);
+  VC_REQUIRE(!s.use_cfg || v_uncond, "ddim_update_frames: CFG needs the unconditional output");
+  VC_REQUIRE(!v_uncond_img || s.use_cfg, "ddim_update_frames: the image-only branch is only defined with CFG on");
+  DdimFrameTable tab;
+  memset(&tab, 0, sizeof(tab));
+  memcpy(tab.f, frames, sizeof(vc_ddim_frame_scalars) * T);
+  const int blocks = ddim_blocks(n, s);
+  if (s.use_cfg && s.guidance_rescale > 0.f) {
+    ddim_stats_kernel<<<blocks, 256, 0, stream>>>(v_cond, v_uncond, v_uncond_img, n, s.cfg_scale, cfg_img, ws);
+    VC_CHECK_CUDA(cudaGetLastError());
+  }
+  ddim_frames_apply_kernel<<<blocks, 256, 0, stream>>>(x, v_cond, v_uncond, v_uncond_img, cfg_img, noise, x_prev, pred_x0, n, T, HW, s,
+                                                       tab, ws, blocks);
   VC_CHECK_CUDA(cudaGetLastError());
   return VC_OK;
 }
@@ -420,8 +499,7 @@ static int dpm_launch(const float* x, const float* v_cond, const float* v_uncond
                       const float* noise, const float* x0_hist1, float* x0_hist, float* x_prev, float* pred_x0, long long n,
                       const vc_ddim_scalars& s, float c_hist, float c_hist2, double* ws, cudaStream_t stream) {
   // the statistics grid of ddim_update (reproducible mode included), so every update reduces the same partial sums in the same order
-  int blocks = (int)min(s.reproducible ? (long long)DDIM_REPRO_BLOCKS : (long long)sm_count() * 4, (n + 255) / 256);
-  if (blocks > DDIM_MAX_BLOCKS) blocks = DDIM_MAX_BLOCKS;
+  const int blocks = ddim_blocks(n, s);
   if (s.use_cfg && s.guidance_rescale > 0.f) {
     ddim_stats_kernel<<<blocks, 256, 0, stream>>>(v_cond, v_uncond, v_uncond_img, n, s.cfg_scale, cfg_img, ws);
     VC_CHECK_CUDA(cudaGetLastError());

@@ -787,6 +787,32 @@ def ddim_update(x, v_cond, v_uncond, noise, sc: dict, v_uncond_img=None, cfg_img
     return x_prev, pred_x0
 
 
+_FRAME_KEYS = ("sqrt_ac_t", "sqrt_1mac_t", "a_prev", "sigma_t", "scale_t", "prev_scale_t")
+
+
+def ddim_update_frames(x, v_cond, v_uncond, noise, sc: dict, frames, v_uncond_img=None, cfg_img: float = 0.0):
+    """ddim_update with a step per frame (vc_ddim_update_frames): x and the predictions are [B', C, T, H, W] fp32 and frame t takes the
+    step scalars frames[t] (a dict with sqrt_ac_t, sqrt_1mac_t, a_prev, sigma_t, scale_t, prev_scale_t); sc holds the per-call
+    cfg_scale and guidance_rescale.  The guidance-rescale stds run over the whole input, as in ddim_update.  T <= 128.  With every
+    frames[t] equal to sc's step scalars the result is ddim_update's bit for bit.  Returns (x_prev, pred_x0)."""
+    for t in (x, v_cond, noise) + ((v_uncond_img,) if v_uncond_img is not None else ()):
+        assert t.dtype == torch.float32 and t.is_contiguous() and t.is_cuda and t.shape == x.shape
+    if x.dim() != 5 or len(frames) != x.shape[2]:
+        raise VcError(f"ddim_update_frames: x must be [B, C, T, H, W] with one entry of `frames` per frame, got {tuple(x.shape)} and "
+                      f"{len(frames)} entries")
+    T, HW = x.shape[2], x.shape[3] * x.shape[4]
+    if T > _lib.DDIM_MAX_FRAMES:
+        raise VcError(f"ddim_update_frames: T={T} unsupported (1..{_lib.DDIM_MAX_FRAMES})")
+    s, use_cfg, ws = _update_args(x, v_uncond, dict(sc, **{k: 0.0 for k in _FRAME_KEYS}))
+    tab = (_lib.DdimFrameScalars * T)(*(_lib.DdimFrameScalars(*(f[k] for k in _FRAME_KEYS)) for f in frames))
+    x_prev, pred_x0 = torch.empty_like(x), torch.empty_like(x)
+    vi = v_uncond_img if use_cfg else None
+    check(_lib.load().vc_ddim_update_frames(x.data_ptr(), v_cond.data_ptr(), _ptr(v_uncond) if use_cfg else None, _ptr(vi),
+                                            float(cfg_img), noise.data_ptr(), x_prev.data_ptr(), pred_x0.data_ptr(), x.numel(), T, HW,
+                                            C.byref(s), tab, ws.data_ptr(), _stream()), "vc_ddim_update_frames")
+    return x_prev, pred_x0
+
+
 def dpm_update(x, v_cond, v_uncond, noise, sc: dict, x0_hist, v_uncond_img=None, cfg_img: float = 0.0):
     """One DPM-Solver++(2M) step (vc_dpm_update): ddim_update's x_{t-1}, plus sc["c_hist"] * (x0 - x0_hist) where x0 is this step's x0
     prediction before the dynamic rescale.  x0_hist (fp32, x's shape) holds the previous step's x0, is read only when c_hist != 0 and

@@ -25,6 +25,7 @@ import contextlib
 
 import torch
 
+from . import fifo as _fifo
 from . import ops, parallel, temporal_window as _tw
 from .ddim import DDIMSampler, check_row_replay
 from .ddim_multiplecond import DDIMSampler as DDIMSampler_multicond
@@ -55,7 +56,7 @@ def get_latent_z(model, videos):
 def image_guided_synthesis(model, prompts, videos, noise_shape, n_samples=1, ddim_steps=50, ddim_eta=1.,
                            unconditional_guidance_scale=1.0, cfg_img=None, fs=None, text_input=False, multiple_cond_cfg=False,
                            timestep_spacing='uniform', guidance_rescale=0.0, condition_index=None, batch_cfg=True, cuda_graph=True,
-                           reproducible=None, sampler="ddim", temporal_window=None, window_seed=0, **kwargs):
+                           reproducible=None, sampler="ddim", temporal_window=None, window_seed=0, fifo=None, **kwargs):
     """reproducible: True / False switches viewcrafter_b200's reproducible mode (ops.set_reproducible) for this call and restores the
     previous setting afterwards; None leaves the process setting as it is.
     sampler: "ddim" (the reference's DDIMSampler), "dpmpp_2m" (dpm_solver.DPMSolverSampler / DPMSolverSamplerMultiCond, which takes
@@ -63,9 +64,22 @@ def image_guided_synthesis(model, prompts, videos, noise_shape, n_samples=1, ddi
     INTEGRATION.md "Samplers").
     temporal_window: None (full temporal attention) or (W, S): the U-Net runs windowed temporal attention for this call and the drawn
     x_T is rescheduled with window_seed (FreeNoise; INTEGRATION.md "Long clips: windowed temporal attention").  The U-Net's previous
-    setting is restored afterwards.  An explicit x_T= is used as given, without rescheduling."""
+    setting is restored afterwards.  An explicit x_T= is used as given, without rescheduling.
+    fifo: None, or a window f (2 <= f <= 128, ddim_steps a multiple of f): FIFO-Diffusion's diagonal denoising (fifo.FIFOSampler /
+    FIFOSamplerMultiCond; INTEGRATION.md "Long clips: FIFO diagonal denoising").  videos and noise_shape carry all N frames while the
+    U-Net only ever runs on f of them, so memory does not grow with N; the latents are decoded f frames at a time.  It runs with
+    sampler="ddim" only, without temporal_window and not on replica groups (ValueError before any work)."""
     if sampler not in SAMPLERS:
         raise ValueError(f"unknown sampler {sampler!r}; choose one of {sorted(SAMPLERS)}")
+    if fifo is not None:
+        if sampler != "ddim":
+            raise ValueError(f"image_guided_synthesis: fifo runs with sampler='ddim' only, got sampler={sampler!r}")
+        if temporal_window is not None:
+            raise ValueError("image_guided_synthesis: fifo and temporal_window cannot be combined (FIFO's U-Net windows are full clips)")
+        if getattr(model, "_replicas", None) is not None:
+            raise ValueError("image_guided_synthesis: fifo does not run on replica groups (parallel.shard_model(replicas=R > 1))")
+        _fifo.check_window(fifo, ddim_steps)
+        kwargs["fifo_window"] = fifo
     if sampler != "ddim":
         SAMPLERS[sampler][0].check_eta(ddim_eta)          # before the conditioning is computed
     with _unet_window(model, _tw.check_window(temporal_window)):
@@ -106,7 +120,9 @@ def _synthesis(model, prompts, videos, noise_shape, n_samples, ddim_steps, ddim_
     unet = getattr(getattr(model, "model", None), "diffusion_model", None)
     if cuda_graph and hasattr(unet, "enable_cuda_graph") and next(unet.parameters()).is_cuda:
         unet.enable_cuda_graph()              # the ~100 forwards of a clip share shapes, weights and context: capture once, replay
-    ddim_sampler = SAMPLERS[sampler][bool(multiple_cond_cfg)](model, batch_cfg=batch_cfg)
+    fifo = kwargs.get("fifo_window")
+    classes = (_fifo.FIFOSampler, _fifo.FIFOSamplerMultiCond) if fifo is not None else SAMPLERS[sampler]
+    ddim_sampler = classes[bool(multiple_cond_cfg)](model, batch_cfg=batch_cfg)
     batch_size = noise_shape[0]
     fs = torch.tensor([fs] * batch_size, dtype=torch.long, device=model.device)
 
@@ -154,8 +170,13 @@ def _synthesis(model, prompts, videos, noise_shape, n_samples, ddim_steps, ddim_
     batch_variants = []
     for _ in range(n_samples):
         samples, _ = ddim_sampler.sample(conditioning=cond, unconditional_conditioning=uc, fs=fs, **options)
-        # latent -> pixel space; on a sharded model every rank decodes its share of the frames (parallel.vae_decode)
-        batch_variants.append(parallel.vae_decode(model, samples) if _vae_sharded(model) else model.decode_first_stage(samples))
+        # latent -> pixel space; on a sharded model every rank decodes its share of the frames (parallel.vae_decode).  FIFO clips are
+        # decoded at most f frames at a time, so the decoder's activations do not grow with the clip either
+        decode = (lambda z: parallel.vae_decode(model, z)) if _vae_sharded(model) else model.decode_first_stage
+        if fifo is None:
+            batch_variants.append(decode(samples))
+        else:
+            batch_variants.append(torch.cat([decode(samples[:, :, i:i + fifo]) for i in range(0, samples.shape[2], fifo)], 2))
     return torch.stack(batch_variants).permute(1, 0, 2, 3, 4, 5)              # batch, variants, c, t, h, w
 
 

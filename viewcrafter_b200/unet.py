@@ -454,8 +454,10 @@ class UNetModel(nn.Module):
     def _res(P, h, skip, emb, B, T, H, W, comm=None):
         BT, HW = B * T, H * W
         a = ops.groupnorm(h, BT, *P["gn1"], 1e-5, True, x2=skip)
-        bias1 = ops.small_linear(emb, P["emb_w"], P["emb_b"], silu_in=True)            # [B, Cout] = emb_layers + conv1 bias
-        h1 = ops.conv3x3(a, BT, H, W, P["w1"], bias=bias1, bias_z_div=T, gn_out=True)      # gn_out: the epilogue leaves the GroupNorm sums of its output
+        # [B, Cout] (one row per sample) or [B*T, Cout] (per-frame timesteps, one row per frame) = emb_layers + conv1 bias
+        bias1 = ops.small_linear(emb, P["emb_w"], P["emb_b"], silu_in=True)
+        # gn_out: the epilogue leaves the GroupNorm sums of its output
+        h1 = ops.conv3x3(a, BT, H, W, P["w1"], bias=bias1, bias_z_div=BT // bias1.shape[0], gn_out=True)
         b = ops.groupnorm(h1, BT, *P["gn2"], 1e-5, True)
         if "skip_w" in P:
             xs = ops.linear(h, P["skip_w"], bias=P["skip_b"], x2=skip)
@@ -628,9 +630,16 @@ class UNetModel(nn.Module):
     @torch.no_grad()
     def forward(self, x, timesteps, context=None, features_adapter=None, fs=None, **kwargs):
         """x [B,in_channels,T,H,W], timesteps [B] long, context [B,L,context_dim], fs [B] long -> [B,out_channels,T,H,W]
-        in x.dtype (openaimodel3d.py:548-603).  Extra kwargs are accepted and ignored like the reference does."""
+        in x.dtype (openaimodel3d.py:548-603).  Extra kwargs are accepted and ignored like the reference does.
+        timesteps may also be [B, T]: one timestep per frame (new functionality, the reference has none; FIFO-Diffusion's diagonal
+        denoising, INTEGRATION.md "Long clips: FIFO diagonal denoising").  Each frame's ResBlocks then take that frame's time
+        embedding (fs is repeated per frame); [B, T] with all timesteps of a sample equal gives the [B] result bit for bit.  Any other
+        shape raises ValueError."""
         if features_adapter is not None:
             _unsupported("features_adapter")
+        B, T = x.shape[0], x.shape[2]
+        if tuple(timesteps.shape) not in ((B,), (B, T)):
+            raise ValueError(f"UNetModel: timesteps must be [B] or [B, T] = [{B}] or [{B}, {T}], got {tuple(timesteps.shape)}")
         if x.is_cuda and context is not None and not torch.cuda.is_current_stream_capturing():
             context = self._canonical_context(context)
             if self._graph_mode:
@@ -640,7 +649,8 @@ class UNetModel(nn.Module):
     def _forward_graphed(self, x, timesteps, context, fs, kwargs):
         ver = ops.tensor_version(context)
         flags = tuple(sorted((k, bool(v)) for k, v in kwargs.items() if k == "cfg_shared_prefix"))
-        key = (tuple(x.shape), x.dtype, id(context), ver, fs is None, flags, id(self._comm), self._twin, self._fp8, ops.reproducible())
+        key = (tuple(x.shape), x.dtype, timesteps.dim(), id(context), ver, fs is None, flags, id(self._comm), self._twin, self._fp8,
+               ops.reproducible())
         e = self._graphs.get(key)
         if ver is None or (e is not None and e["ctx"] is not context):
             return self._forward_impl(x, timesteps, context, fs, kwargs)
@@ -696,16 +706,24 @@ class UNetModel(nn.Module):
         # and c_concat and differ only in the cross-attention context
         kinds = [Pm["kind"] for Pm in P["input"][1]] if len(P["input"]) > 1 else []
         shared = bool(kwargs.get("cfg_shared_prefix")) and B >= 2 and comm is None and kinds[:2] == ["R", "S"]
-        # --- embeddings (fp32) : time_embed(t) + fps_embedding(fs), one row per batch element (frame-invariant) ---
+        # --- embeddings (fp32) : time_embed(t) + fps_embedding(fs), one row per batch element (frame-invariant), or with [B, T]
+        # timesteps one row per (batch element, frame) of all T_all frames, fs repeated per frame ---
         ts = timesteps.to(device=dev, dtype=torch.int64).contiguous()
+        per_frame_t = ts.dim() == 2
         tw = P["time"]
-        emb = ops.small_linear(ops.small_linear(ops.timestep_embedding(ts, self.model_channels), tw[0], tw[1]), tw[2], tw[3], silu_in=True)
+        emb = ops.small_linear(ops.small_linear(ops.timestep_embedding(ts.reshape(-1), self.model_channels), tw[0], tw[1]), tw[2], tw[3],
+                               silu_in=True)
         if self.fs_condition:
             if fs is None:
                 fs = torch.full((B,), self.default_fs, dtype=torch.int64, device=dev)
+            fs = fs.to(device=dev, dtype=torch.int64)
+            if per_frame_t:
+                fs = fs.repeat_interleave(T_all)
             fw = P["fps"]
-            fs_h = ops.small_linear(ops.timestep_embedding(fs.to(device=dev, dtype=torch.int64).contiguous(), self.model_channels), fw[0], fw[1])
+            fs_h = ops.small_linear(ops.timestep_embedding(fs.contiguous(), self.model_channels), fw[0], fw[1])
             emb = ops.small_linear(fs_h, fw[2], fw[3], silu_in=True, add=emb)
+        if per_frame_t and comm:                   # this rank's frames [f0, f1)
+            emb = emb.view(B, T_all, -1)[:, f0:f1].reshape(B * T, -1).contiguous()
         # --- context: text[:77] | image tokens; per-frame image tokens when L == 77 + 16*T (openaimodel3d.py:556-560) ---
         ctx16 = ops.cast_f16(context.float().contiguous())
         L = context.shape[1]
@@ -725,7 +743,7 @@ class UNetModel(nn.Module):
             # SURVEY.md App. C.2: all CFG branches see the same x, t, fs and c_concat, so everything before the first
             # cross-attention (input_blocks.0, init_attn, input_blocks.1.0 and input_blocks.1.1 up to attn1) is computed once
             # on one batch element and copied B times; the results are those of the plain batch-B forward.
-            emb1 = emb[:1].contiguous()
+            emb1 = emb[:emb.shape[0] // B].contiguous()     # sample 0's row (or its T rows with [B, T] timesteps)
             h = h[:T * H * W]
             h, H, W = self._run_stage(P["input"][0], h, None, emb1, ctx, 1, T, H, W)
             if self.addition_attention:
