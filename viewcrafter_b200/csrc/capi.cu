@@ -26,8 +26,9 @@ void vc_reset_launch_count(void) { vc::g_launches.store(0); }
 
 int vc_gemm_tap(const vc_gemm_desc* d, void* stream) {
   if (!d) { set_error("vc_gemm_tap: null descriptor"); return VC_ERR_ARG; }
-  COUNT(1);
-  return gemm_tap(*d, ST(stream));
+  const int rc = gemm_tap(*d, ST(stream));
+  if (rc == VC_OK) COUNT(1);                  // a descriptor refused on the host launches nothing
+  return rc;
 }
 int vc_gemm_tile_n(int32_t N, int32_t geglu) { return vc::pick_bn_public(N, geglu); }
 int vc_absmax_f16(const void* x1, int64_t rows, int32_t cols1, int32_t ld1, const void* x2, int32_t cols2, int32_t ld2, float* amax,

@@ -17,6 +17,7 @@
 // when the kernel ends, the data of all peers has landed.  Receive buffers are reused: a rank can only be writing collective
 // s into a peer's buffer after that peer signalled s-1, which in the peer's stream order comes after every reader of the
 // previous contents (the two directions use different buffers and strictly alternate).
+#include <atomic>
 #include <cstring>
 
 #include "common.cuh"
@@ -183,10 +184,14 @@ __global__ void __launch_bounds__(512) peer_exchange_kernel(const __grid_constan
   }
   __syncthreads();
   if (!is_last) return;
+  // the split records are summed in fp64 and rounded once, as gn_finalize_kernel and the apply pass sum them: an fp32 running sum
+  // over the splits loses enough of the sum of squares to push the rstd error of offset groups past the split form's
   float mine = 0.f;
   if (p.with_stats && tid < p.B * 64) {
     const int bb = tid >> 6, t = tid & 63;
-    for (int spx = 0; spx < p.splits; ++spx) mine += __ldcg(p.partial + ((long long)bb * p.splits + spx) * 64 + t);
+    double acc = 0.0;
+    for (int spx = 0; spx < p.splits; ++spx) acc += __ldcg(p.partial + ((long long)bb * p.splits + spx) * 64 + t);
+    mine = (float)acc;
   }
   peer_finish(p.pc, p.B, p.with_stats != 0, mine, tid);
 }
@@ -197,9 +202,11 @@ __global__ void __launch_bounds__(512) peer_exchange_kernel(const __grid_constan
 __global__ void __launch_bounds__(PEER_ALLREDUCE_THREADS) gn_peer_allreduce_kernel(const float* __restrict__ partial, int splits, int B, const __grid_constant__ PeerCommDev pc) {
   const int tid = threadIdx.x;
   float mine = 0.f;
-  if (tid < B * 64) {
+  if (tid < B * 64) {                                  // fp64 over the splits, rounded once (see peer_exchange_kernel)
     const int b = tid >> 6, t = tid & 63;
-    for (int sp = 0; sp < splits; ++sp) mine += partial[((long long)b * splits + sp) * 64 + t];
+    double acc = 0.0;
+    for (int sp = 0; sp < splits; ++sp) acc += partial[((long long)b * splits + sp) * 64 + t];
+    mine = (float)acc;
   }
   peer_finish(pc, B, B > 0, mine, tid);
 }
@@ -237,6 +244,7 @@ __global__ void __launch_bounds__(512) peer_leaves_kernel(const float* __restric
 
 // ------------------------------------------------------------------------------------------------------------------
 namespace vc {
+extern std::atomic<long long> g_launches;      // vc_launch_count: kernels launched, counted once they are enqueued
 int groupnorm_stats_partials(const __half* x1, int C1, int samples, long long rows_per_sample, float* partial_ws, size_t ws_bytes,
                              int* splits_out, cudaStream_t stream);
 
@@ -343,6 +351,7 @@ int vc_peer_exchange(const vc_peer_comm* c, const void* src, void* const* dst, i
   dim3 grid(splits, B);
   peer_exchange_kernel<<<grid, p.vecs * p.ppi, p.with_stats ? (size_t)2 * C * p.ppi * sizeof(float) : 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
   VC_CHECK_CUDA(cudaGetLastError());
+  g_launches.fetch_add(1, std::memory_order_relaxed);
   return VC_OK;
 }
 
@@ -359,6 +368,7 @@ int vc_peer_groupnorm_stats(const vc_peer_comm* c, const void* x, int32_t C, int
   if (rc) return rc;
   gn_peer_allreduce_kernel<<<1, PEER_ALLREDUCE_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(reinterpret_cast<const float*>(ws), splits, samples, d);
   VC_CHECK_CUDA(cudaGetLastError());
+  g_launches.fetch_add(2, std::memory_order_relaxed);
   return VC_OK;
 }
 
@@ -380,6 +390,7 @@ int vc_peer_finish_scatter(const vc_peer_comm* c, const vc_gn_part_geom* geom, i
   }
   gn_peer_allreduce_kernel<<<1, PEER_ALLREDUCE_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(reinterpret_cast<const float*>(ws), splits, B, d);
   VC_CHECK_CUDA(cudaGetLastError());
+  g_launches.fetch_add(geom ? 2 : 1, std::memory_order_relaxed);
   return VC_OK;
 }
 
@@ -399,6 +410,7 @@ int vc_peer_gather_leaves(const vc_peer_comm* c, const float* leaves, void* cons
   }
   peer_leaves_kernel<<<1, 512, 0, reinterpret_cast<cudaStream_t>(stream)>>>(leaves, ld, cap, B, T, nc, gathered, d);
   VC_CHECK_CUDA(cudaGetLastError());
+  g_launches.fetch_add(1, std::memory_order_relaxed);
   return VC_OK;
 }
 

@@ -347,15 +347,8 @@ class PeerFrameComm(FrameComm):
         into the receive buffers of the ranks that own them in the other layout (TMA stores over NVLink, overlapped with its MMAs), and
         a one-CTA kernel completes the switch (rendezvous + the cross-rank GroupNorm sums from the GEMM's own partial sums).  Replaces
         GEMM -> local tensor -> peer_exchange_kernel.  None when the shape is not supported (the caller then switches separately)."""
-        P = self.world
-        if self.fused == "0" or P > min(4, self.fused_max_p) or HW % P != 0 or Cc % 32 != 0 or B > self.bmax:
+        if not fused_scatter_ok(self.fused, self.fused_max_p, self.bmax, self.ranges, B, HW, Cc):
             return None
-        if self.fused == "aligned" and ((HW // P) % 32 != 0 or HW % 32 != 0):
-            return None
-        # the decision must be the same on every rank of the group: it depends on ALL frame ranges, not on this rank's
-        for f0, f1 in self.ranges:
-            if f1 - f0 == 0 or (B > 1 and ((f1 - f0) * HW) % 128 != 0):
-                return None
         return _ScatterPlan(self, to_sites, B, HW, Cc)
 
     def owns(self, t: torch.Tensor) -> bool:
@@ -370,6 +363,22 @@ class PeerFrameComm(FrameComm):
         for p in self._own_ptrs:
             self.lib.vc_peer_free(p)
         self._peer_ptrs, self._own_ptrs, self._bufs, self._leaves = [], [], {}, None
+
+
+def fused_scatter_ok(fused: str, fused_max_p: int, bmax: int, ranges, B: int, HW: int, Cc: int) -> bool:
+    """Whether a layout switch of B samples of HW pixels and Cc channels over a frame group with the frame ranges `ranges` (one per
+    rank) may run in the producing GEMM's epilogue (PeerFrameComm.scatter_plan).  `fused`, `fused_max_p`: PeerFrameComm's settings
+    (VC_PEER_FUSED, VC_PEER_FUSED_MAXP); bmax: the largest batch of the group's buffers."""
+    P = len(ranges)
+    if fused == "0" or P > min(4, fused_max_p) or HW % P != 0 or Cc % 32 != 0 or B > bmax:
+        return False
+    if fused == "aligned" and ((HW // P) % 32 != 0 or HW % 32 != 0):
+        return False
+    # the decision must be the same on every rank of the group: it depends on ALL frame ranges, not on this rank's
+    for f0, f1 in ranges:
+        if f1 - f0 == 0 or (B > 1 and ((f1 - f0) * HW) % 128 != 0):
+            return False
+    return True
 
 
 class _ScatterPlan:
