@@ -15,6 +15,7 @@ from typing import List
 
 import torch
 
+from . import _lib, ops
 from .distributions import posterior_class
 
 
@@ -30,6 +31,8 @@ def frame_ranges(T: int, world: int) -> List[tuple]:
 
 
 class FrameComm:
+    identity_switches = False       # True: to_sites / to_frames return their argument, with the GroupNorm sums its producer left on it
+
     def __init__(self, dist, rank: int, world: int, group=None):
         self.dist, self.rank, self.world, self.group = dist, rank, world, group
         self.T = None
@@ -118,10 +121,12 @@ class FrameComm:
         """No fused switch with NCCL collectives (see PeerFrameComm.scatter_plan): the caller switches separately."""
         return None
 
+    def owns(self, t: torch.Tensor) -> bool:
+        return False
+
     def groupnorm5d(self, x, B, gamma, beta, eps, silu, stat_rows, fresh: bool):
         """GroupNorm(32) of a site-layout tensor whose statistics span the ranks of the group.  `fresh`: x is the tensor the
         last to_sites() returned (the peer-memory path already holds its statistics)."""
-        from . import ops
         if ops.reproducible():
             return self._groupnorm5d_leaves(x, B, gamma, beta, eps, silu, stat_rows)
         st = ops.groupnorm_stats(x, B)
@@ -134,7 +139,6 @@ class FrameComm:
     def leaf_geometry(self, stat_rows: int):
         """(HW, nc, rows per leaf) of a site-layout 5-D GroupNorm over stat_rows = T * HW rows per sample: this rank holds the chunks
         [rank * nc / P, (rank + 1) * nc / P) of every frame, whole, so its leaves are exactly those of a single GPU."""
-        from . import ops
         HW = stat_rows // self.T
         nc = ops.gn_leaf_chunks(HW)
         if nc % self.world != 0:
@@ -153,7 +157,6 @@ class FrameComm:
         return parts.view(P, B * self.T, ncl, 64).permute(1, 0, 2, 3).reshape(B * self.T * nc, 32, 2).contiguous()
 
     def _groupnorm5d_leaves(self, x, B, gamma, beta, eps, silu, stat_rows):
-        from . import ops
         HW, nc, rows_per_leaf = self.leaf_geometry(stat_rows)
         leaves = self.gather_leaves(ops.groupnorm_leaves(x, rows_per_leaf), B, nc)
         return ops.groupnorm_apply_leaves(x, B, leaves, stat_rows, gamma, beta, eps, silu)
@@ -167,6 +170,24 @@ class FrameComm:
         parts = y_local.new_empty((self.world, B, C, tmax, H, W))
         self.dist.all_gather_into_tensor(parts.view(-1), mine.view(-1), group=self.group)       # uneven frame counts: padded to the largest shard
         return torch.cat([parts[r, :, :, :f1 - f0] for r, (f0, f1) in enumerate(self.ranges)], dim=2)
+
+
+class LocalFrameComm(FrameComm):
+    """The frame group of one GPU, which UNetModel runs through when it is not frame-sharded over several: it owns all T frames, its
+    layout switches and frame gather return their argument, and its 5-D GroupNorm takes its statistics locally.  Opens no process group."""
+    identity_switches = True
+
+    def __init__(self):
+        super().__init__(None, 0, 1)
+
+    def to_sites(self, h: torch.Tensor, *_) -> torch.Tensor:
+        return h
+    to_frames = gather_frames = to_sites
+
+    def groupnorm5d(self, x, B, gamma, beta, eps, silu, stat_rows, fresh: bool):
+        if ops.reproducible():
+            return ops.groupnorm_canonical(x, B, stat_rows // self.T, gamma, beta, eps, silu)
+        return ops.groupnorm(x, B, gamma, beta, eps, silu)
 
 
 class PeerFrameComm(FrameComm):
@@ -184,7 +205,6 @@ class PeerFrameComm(FrameComm):
 
     def __init__(self, dist, rank: int, world: int, group, device, bmax: int = 4):
         super().__init__(dist, rank, world, group)
-        from . import _lib
         self.lib = _lib.load()
         self.device = torch.device(device)
         self.bmax = bmax
@@ -228,7 +248,6 @@ class PeerFrameComm(FrameComm):
         `dtype`, [device pointer of rank q's allocation as mapped into this process]); the mapping is opened with this rank's
         compute device current, which is what gives its kernels access over NVLink."""
         import ctypes as C
-        from . import _lib
         nbytes = (int(nbytes) + 255) // 256 * 256
         ptr, handle = C.c_void_p(), (C.c_uint8 * 64)()
         _lib.check(self.lib.vc_peer_alloc(nbytes, C.byref(ptr), handle), "vc_peer_alloc")
@@ -265,7 +284,6 @@ class PeerFrameComm(FrameComm):
 
     def _exchange(self, h: torch.Tensor, B: int, HW: int, to_sites: bool) -> torch.Tensor:
         import ctypes as C
-        from . import _lib
         P, Cc = self.world, h.shape[1]
         assert HW % P == 0, f"H*W={HW} must be divisible by the world size {P}"
         assert h.is_contiguous() and h.dtype == torch.float16 and B <= self.bmax
@@ -277,7 +295,6 @@ class PeerFrameComm(FrameComm):
         own, ptrs, _ = self._buffer("sites" if to_sites else "frames", cap)
         dst = (C.c_void_p * P)(*ptrs)
         f0 = (C.c_int32 * (P + 1))(*([r[0] for r in self.ranges] + [self.T]))
-        from . import ops
         with_stats = to_sites and not ops.reproducible()          # reproducible mode takes its statistics from leaves
         _lib.check(self.lib.vc_peer_exchange(C.byref(self.c), h.data_ptr(), dst, int(to_sites), B, self.T, HW, Cc, f0, int(with_stats),
                                              self.ws.data_ptr(), self.ws.numel() * 4, torch.cuda.current_stream().cuda_stream), "vc_peer_exchange")
@@ -297,7 +314,6 @@ class PeerFrameComm(FrameComm):
         """FrameComm.gather_leaves through peer memory: one kernel stores this rank's leaves into their canonical place of every rank's
         leaf buffer and, after the rendezvous, copies the gathered array out (graph-capturable, no NCCL call)."""
         import ctypes as C
-        from . import _lib
         n = B * self.T * nc * 64
         own, ptrs, cap = self._leaf_buffer(n)
         out = torch.empty((B * self.T * nc, 32, 2), device=leaves.device, dtype=torch.float32)
@@ -323,7 +339,6 @@ class PeerFrameComm(FrameComm):
 
     def groupnorm5d(self, x, B, gamma, beta, eps, silu, stat_rows, fresh: bool):
         import ctypes as C
-        from . import _lib, ops
         if ops.reproducible():
             self._stats_of = None
             return self._groupnorm5d_leaves(x, B, gamma, beta, eps, silu, stat_rows)
@@ -385,7 +400,6 @@ class _ScatterPlan:
     """One fused layout switch (PeerFrameComm.scatter_plan): attach() fills the GEMM descriptor, finish() completes the switch."""
 
     def __init__(self, comm: "PeerFrameComm", to_sites: bool, B: int, HW: int, Cc: int):
-        from . import _lib
         self.comm, self.to_sites, self.B, self.HW, self.C = comm, to_sites, B, HW, Cc
         P = comm.world
         HWl = HW // P
@@ -412,7 +426,6 @@ class _ScatterPlan:
     def finish(self, gn_part):
         """Rendezvous (+ cross-rank GroupNorm sums for frames -> sites).  Returns the switched tensor (a view of the receive buffer)."""
         import ctypes as C
-        from . import _lib
         comm = self.comm
         geom = None
         if self.to_sites and gn_part is not None:
@@ -596,7 +609,6 @@ def shard_model(model, dist, rank: int, world: int, cfg_split: bool = True, peer
         device = next(unet.parameters()).device
     except StopIteration:
         device = None
-    from . import ops
     modes = [None] * world
     dist.all_gather_object(modes, (ops.reproducible(), replicas))
     if len(set(m for m, _ in modes)) != 1:
@@ -614,7 +626,6 @@ def shard_model(model, dist, rank: int, world: int, cfg_split: bool = True, peer
         raise ValueError(f"shard_model: reproducible mode supports frame groups of 1, 2, 4 or 8 GPUs (they divide the GroupNorm chunks "
                          f"of every frame); this layout puts {P} GPUs in a frame group")
     if peer is None:           # NVLink peer-memory kernels on CUDA (VC_PEER_COMM=0: NCCL collectives); the CPU double uses gloo
-        import os
         peer = os.environ.get("VC_PEER_COMM", "1") != "0"
     if getattr(model, "first_stage_model", None) is not None:
         model._vae_comm = FrameComm(dist, rank, world)

@@ -21,7 +21,7 @@ from typing import List, Optional
 import torch
 import torch.nn as nn
 
-from . import ops, temporal_window
+from . import ops, parallel, temporal_window
 
 
 def _zero(m: nn.Module) -> nn.Module:
@@ -451,7 +451,7 @@ class UNetModel(nn.Module):
     # block executors (operate on row matrices)
     # ------------------------------------------------------------------------------------------
     @staticmethod
-    def _res(P, h, skip, emb, B, T, H, W, comm=None):
+    def _res(P, h, skip, emb, B, T, H, W, comm):
         BT, HW = B * T, H * W
         a = ops.groupnorm(h, BT, *P["gn1"], 1e-5, True, x2=skip)
         # [B, Cout] (one row per sample) or [B*T, Cout] (per-frame timesteps, one row per frame) = emb_layers + conv1 bias
@@ -463,32 +463,22 @@ class UNetModel(nn.Module):
             xs = ops.linear(h, P["skip_w"], bias=P["skip_b"], x2=skip)
         else:
             xs = h
-        # multi-GPU: the frames -> sites switch the TemporalConvBlock needs is performed by conv2's own epilogue when the peer-memory path
-        # offers a plan (its output tiles go straight to the owning ranks), and the switch back by the last temporal conv's
-        to_s = comm.scatter_plan(True, B, HW, P["w2"].shape[0] // 9) if (comm and "tconv" in P) else None
+        # the frames -> sites switch the TemporalConvBlock needs is performed by conv2's own epilogue when the frame group offers a plan
+        # (its output tiles go straight to the owning ranks), and the switch back by the last temporal conv's
+        to_s = comm.scatter_plan(True, B, HW, P["w2"].shape[0] // 9) if "tconv" in P else None
         h2 = ops.conv3x3(b, BT, H, W, P["w2"], bias=P["b2"], res=xs, gn_out=True, peer=to_s)
         if "tconv" in P:
-            # TemporalConvBlock: needs every frame of a pixel -> (optionally) transpose frames<->sites across GPUs
-            t = ident = h2 if to_s is not None else (comm.to_sites(h2, B, HW) if comm else h2)
-            Tg, HWl = (comm.T, HW // comm.world) if comm else (T, HW)
+            # TemporalConvBlock: needs every frame of a pixel -> the site layout (all T frames of H*W / world pixels)
+            t = ident = h2 if to_s is not None else comm.to_sites(h2, B, HW)
+            Tg, HWl = comm.T, HW // comm.world
             n_tc, to_f = len(P["tconv"]), None
             for i, (g, be, w3, b3) in enumerate(P["tconv"]):
-                t = UNetModel._gn5d(t, B, g, be, 1e-5, True, comm, Tg * HW, HW, fresh=(i == 0))   # statistics over (C/32, T, H, W)
+                t = comm.groupnorm5d(t, B, g, be, 1e-5, True, Tg * HW, fresh=(i == 0))     # statistics over (C/32, T, H, W)
                 last = i == n_tc - 1
-                to_f = comm.scatter_plan(False, B, HW, w3.shape[0] // 3) if (comm and last) else None
-                t = ops.conv_temporal(t, B, Tg, HWl, w3, bias=b3, res=ident if last else None, gn_out=comm is None, peer=to_f)
-            h2 = t if to_f is not None else (comm.to_frames(t, B, HW) if comm else t)
+                to_f = comm.scatter_plan(False, B, HW, w3.shape[0] // 3) if last else None
+                t = ops.conv_temporal(t, B, Tg, HWl, w3, bias=b3, res=ident if last else None, gn_out=comm.identity_switches, peer=to_f)
+            h2 = t if to_f is not None else comm.to_frames(t, B, HW)
         return h2
-
-    @staticmethod
-    def _gn5d(x, B, gamma, beta, eps, silu, comm, stat_rows, hw, fresh=False):
-        """GroupNorm whose statistics span all frames of hw pixels (and, when sharded, all GPUs: [B,32,2] partial sums are exchanged --
-        riding on the layout switch when `fresh`, i.e. x is what comm.to_sites() just returned; canonical leaves in reproducible mode)."""
-        if not comm:
-            if ops.reproducible():
-                return ops.groupnorm_canonical(x, B, hw, gamma, beta, eps, silu)
-            return ops.groupnorm(x, B, gamma, beta, eps, silu)
-        return comm.groupnorm5d(x, B, gamma, beta, eps, silu, stat_rows, fresh)
 
     @staticmethod
     def _spatial_tf(P, h, ctx, B, T, H, W, expand=False, out_plan=None):
@@ -524,16 +514,15 @@ class UNetModel(nn.Module):
         return ops.linear(x, P["out_w"], bias=P["out_b"], res=h, gn_out=True, peer=out_plan)
 
     @staticmethod
-    def _temporal_tf(P, h, B, T, H, W, comm=None, pre_sites=False, window=None):
+    def _temporal_tf(P, h, B, H, W, comm, pre_sites=False, window=None):
         """pre_sites: `h` already is in the site layout (the producing GEMM switched it, see _spatial_tf(out_plan=...)).
         window: (W, S) of set_temporal_window or None.  Under frame sharding each rank holds all frames of its sites, so the
         windows are local too."""
         HW, heads = H * W, P["heads"]
         C = heads * 64
-        Tg, HWl = (comm.T, HW // comm.world) if comm else (T, HW)
-        t_in = h if pre_sites else (comm.to_sites(h, B, HW) if comm else h)
-        x, st = ops.linear(UNetModel._gn5d(t_in, B, *P["gn"], 1e-6, False, comm, Tg * HW, HW, fresh=True), P["in_w"], bias=P["in_b"],
-                           ln_out=True)
+        Tg, HWl = comm.T, HW // comm.world
+        t_in = h if pre_sites else comm.to_sites(h, B, HW)
+        x, st = ops.linear(comm.groupnorm5d(t_in, B, *P["gn"], 1e-6, False, Tg * HW, fresh=True), P["in_w"], bias=P["in_b"], ln_out=True)
         for Q in P["blocks"]:
             for wqkv, ow, ob in (("qkv1", "o1_w", "o1_b"), ("qkv2", "o2_w", "o2_b")):
                 qkv = _ln_linear(Q, x, st, wqkv)
@@ -547,12 +536,12 @@ class UNetModel(nn.Module):
                         ops.temporal_attn(qkv[rows, :C], qkv[rows, C:2 * C], qkv[rows, 2 * C:], Tg, HWl, heads, out=a[rows])
                 x, st = ops.linear(a, Q[ow], bias=Q[ob], res=x, ln_out=True)
             x, st = _ff(Q, x, st, Q is P["blocks"][-1])
-        to_f = comm.scatter_plan(False, B, HW, P["out_w"].shape[0]) if comm else None
-        out = ops.linear(x, P["out_w"], bias=P["out_b"], res=t_in, gn_out=comm is None, peer=to_f)
-        return out if to_f is not None else (comm.to_frames(out, B, HW) if comm else out)
+        to_f = comm.scatter_plan(False, B, HW, P["out_w"].shape[0])
+        out = ops.linear(x, P["out_w"], bias=P["out_b"], res=t_in, gn_out=comm.identity_switches, peer=to_f)
+        return out if to_f is not None else comm.to_frames(out, B, HW)
 
-    def _run_stage(self, stage, h, skip, emb, ctx, B, T, H, W):
-        comm, pre_sites = self._comm, False
+    def _run_stage(self, stage, h, skip, emb, ctx, comm, B, T, H, W):
+        pre_sites = False
         for idx, P in enumerate(stage):
             k = P["kind"]
             if k == "R":
@@ -560,11 +549,11 @@ class UNetModel(nn.Module):
                 skip = None
             elif k == "S":
                 nxt = stage[idx + 1]["kind"] if idx + 1 < len(stage) else None
-                plan = comm.scatter_plan(True, B, H * W, P["out_w"].shape[0]) if (comm and nxt == "T") else None
+                plan = comm.scatter_plan(True, B, H * W, P["out_w"].shape[0]) if nxt == "T" else None
                 h = self._spatial_tf(P, h, ctx, B, T, H, W, out_plan=plan)
                 pre_sites = plan is not None
             elif k == "T":
-                h = self._temporal_tf(P, h, B, T, H, W, comm, pre_sites=pre_sites, window=self._twin)
+                h = self._temporal_tf(P, h, B, H, W, comm, pre_sites=pre_sites, window=self._twin)
                 pre_sites = False
             elif k == "D":
                 cols, H, W = ops.im2col_s2(h, B * T, H, W)
@@ -668,8 +657,8 @@ class UNetModel(nn.Module):
             g = torch.cuda.CUDAGraph()
             n0 = ops.launch_count()
             with torch.cuda.graph(g, capture_error_mode="thread_local"):
-                # the final frame gather is a NCCL collective: keep it out of the capture (the peer-memory exchanges are plain kernels)
-                e["out"] = self._forward_impl(e["x"], e["t"], context, e["fs"], kwargs, gather=False)
+                # a sharded forward's final frame gather is a NCCL collective: keep it out of the capture (peer exchanges are kernels)
+                e["out"] = self._forward_impl(e["x"], e["t"], context, e["fs"], kwargs, gather=not self._comm)
             e["graph"] = g
             e["launches"] = ops.launch_count() - n0     # kernels of this library inside the graph (launched again by every replay)
             e["kv"] = list(self._kv_caches)             # the captured kernels read these K/V projections: keep them alive
@@ -694,18 +683,18 @@ class UNetModel(nn.Module):
         P = self._packs()
         if P["device"] != x.device:
             raise ops.VcError(f"UNetModel weights are on {P['device']} but the input is on {x.device}")
-        comm = self._comm
+        # frame sharding: this rank owns frames [f0, f1) for every spatial op (one GPU: all of them)
+        comm = self._comm or parallel.LocalFrameComm()
         T_all = x.shape[2]
-        if comm:                                   # frame sharding: this rank owns frames [f0, f1) for every spatial op
-            f0, f1 = comm.bind(T_all)
-            x_full, x = x, x[:, :, f0:f1]
+        f0, f1 = comm.bind(T_all)
+        x = x[:, :, f0:f1]
         B, Cin, T, H, W = x.shape
         dev = x.device
         x32 = x.float().contiguous()
         # cfg_shared_prefix: the caller (DDIMSampler._apply_stacked) asserts that all B batch rows carry the same x, t, fs
         # and c_concat and differ only in the cross-attention context
         kinds = [Pm["kind"] for Pm in P["input"][1]] if len(P["input"]) > 1 else []
-        shared = bool(kwargs.get("cfg_shared_prefix")) and B >= 2 and comm is None and kinds[:2] == ["R", "S"]
+        shared = bool(kwargs.get("cfg_shared_prefix")) and B >= 2 and self._comm is None and kinds[:2] == ["R", "S"]
         # --- embeddings (fp32) : time_embed(t) + fps_embedding(fs), one row per batch element (frame-invariant), or with [B, T]
         # timesteps one row per (batch element, frame) of all T_all frames, fs repeated per frame ---
         ts = timesteps.to(device=dev, dtype=torch.int64).contiguous()
@@ -722,13 +711,13 @@ class UNetModel(nn.Module):
             fw = P["fps"]
             fs_h = ops.small_linear(ops.timestep_embedding(fs.contiguous(), self.model_channels), fw[0], fw[1])
             emb = ops.small_linear(fs_h, fw[2], fw[3], silu_in=True, add=emb)
-        if per_frame_t and comm:                   # this rank's frames [f0, f1)
+        if per_frame_t:                            # this rank's frames [f0, f1)
             emb = emb.view(B, T_all, -1)[:, f0:f1].reshape(B * T, -1).contiguous()
         # --- context: text[:77] | image tokens; per-frame image tokens when L == 77 + 16*T (openaimodel3d.py:556-560) ---
         ctx16 = ops.cast_f16(context.float().contiguous())
         L = context.shape[1]
         per_frame = (L == 77 + T_all * 16)
-        img_lo, img_hi = (77 + 16 * f0, 77 + 16 * f1) if (comm and per_frame) else (77, L)
+        img_lo, img_hi = (77 + 16 * f0, 77 + 16 * f1) if per_frame else (77, L)
         ctx = dict(text=[ctx16[b, :77] for b in range(B)], img=[ctx16[b, img_lo:img_hi] for b in range(B)] if L > 77 else None,
                    img_per_frame=per_frame, kv=self._kv_projector(context, (img_lo, img_hi)))
         # --- input latent -> rows [(b t) h w, Cin padded to 8] ---
@@ -745,37 +734,34 @@ class UNetModel(nn.Module):
             # on one batch element and copied B times; the results are those of the plain batch-B forward.
             emb1 = emb[:emb.shape[0] // B].contiguous()     # sample 0's row (or its T rows with [B, T] timesteps)
             h = h[:T * H * W]
-            h, H, W = self._run_stage(P["input"][0], h, None, emb1, ctx, 1, T, H, W)
+            h, H, W = self._run_stage(P["input"][0], h, None, emb1, ctx, comm, 1, T, H, W)
             if self.addition_attention:
-                h, H, W = self._run_stage(P["init_attn"], h, None, emb1, ctx, 1, T, H, W)
+                h, H, W = self._run_stage(P["init_attn"], h, None, emb1, ctx, comm, 1, T, H, W)
             hs.append(torch.cat([h] * B, 0))
             Bc = 1
             for Pm in P["input"][1]:
-                if Bc == 1 and Pm["kind"] == "R":
-                    h = self._res(Pm, h, None, emb1, 1, T, H, W, None)
-                elif Bc == 1 and Pm["kind"] == "S":
+                if Bc == 1 and Pm["kind"] == "S":
                     h = self._spatial_tf(Pm, h, ctx, B, T, H, W, expand=True)
                     Bc = B
                 else:
-                    h, H, W = self._run_stage([Pm], h, None, emb, ctx, B, T, H, W)
+                    h, H, W = self._run_stage([Pm], h, None, emb1 if Bc == 1 else emb, ctx, comm, Bc, T, H, W)
             hs.append(h)
             first = 2
         for i, stage in enumerate(P["input"]):
             if i < first:
                 continue
-            h, H, W = self._run_stage(stage, h, None, emb, ctx, B, T, H, W)
+            h, H, W = self._run_stage(stage, h, None, emb, ctx, comm, B, T, H, W)
             if i == 0 and self.addition_attention:
-                h, H, W = self._run_stage(P["init_attn"], h, None, emb, ctx, B, T, H, W)
-            if comm and getattr(comm, "owns", None) and comm.owns(h):
+                h, H, W = self._run_stage(P["init_attn"], h, None, emb, ctx, comm, B, T, H, W)
+            if comm.owns(h):
                 h = h.clone()                      # a skip outlives the reusable peer receive buffer it was delivered in
             hs.append(h)
-        h, H, W = self._run_stage(P["middle"], h, None, emb, ctx, B, T, H, W)
+        h, H, W = self._run_stage(P["middle"], h, None, emb, ctx, comm, B, T, H, W)
         for stage in P["output"]:
-            h, H, W = self._run_stage(stage, h, hs.pop(), emb, ctx, B, T, H, W)
+            h, H, W = self._run_stage(stage, h, hs.pop(), emb, ctx, comm, B, T, H, W)
         y = ops.conv3x3(ops.groupnorm(h, B * T, *P["out_gn"], 1e-5, True), B * T, H, W, P["out_w"], bias=P["out_b"], out_f32=True)
         out = ops.rows_to_ncthw(y, B, self.out_channels, T, H, W)
-        if comm:                                   # every rank needs the whole prediction for the (global-std) DDIM update
-            if not gather:
-                return out                            # this rank's frames only (the graph path gathers after the replay)
-            out = comm.gather_frames(out, T_all)
-        return out.to(x.dtype)
+        if not gather:
+            return out                             # this rank's frames only (the graph path gathers after the replay)
+        # every rank needs the whole prediction for the (global-std) DDIM update
+        return comm.gather_frames(out, T_all).to(x.dtype)
